@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - training rays/s of the LiDAR4D hot path on B200 (driver contract in the task brief).
+"""bench.py - training rays/s of the LiDAR4D hot path on one H100 (or several, under torchrun).
 
 Workload (BASELINE.json configs[1]): synthetic KITTI-360-like sweep of 64x1024 rays x 768 samples,
 L=16 4D hash + 6 hex-planes + flow field, 50-frame straight trajectory (SURVEY.md 8(d)).
@@ -8,6 +8,7 @@ fused kernels over the sweep (in ray chunks, gradients accumulated), one Adam st
 reference's recipe (main_lidar4d.py:298-300) and the re-staging of the kernel working set.
 
   python bench.py [--gpus N --steps K --warmup W]            this repo's CUDA path
+  python bench.py ... --dump-outputs DIR                     also write what the last timed step computed as DIR/<name>.npy
   python bench.py --impl reference [...]                     CPU reference arm: the oracle port of the
                                                              reference python path (tiny-cuda-nn cannot run
                                                              anywhere here), bounded sample per step
@@ -62,6 +63,10 @@ def parse():
     ap.add_argument("--pipeline", default="split", choices=["split", "fused"])
     ap.add_argument("--mlp", default="fp16", choices=["fp16", "fp32"],
                     help="fp16: MLP weights as fp16 working copies (as tiny-cuda-nn), tensor-core dense kernels; fp32: FMA")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (per-ray depth and image, the loss, the "
+                         "updated sigma-MLP weights and a fixed sample of the updated hash tables) as DIR/<name>.npy; the inputs "
+                         "depend only on the arguments, so two builds can be compared output for output")
     return ap.parse_args()
 
 
@@ -117,7 +122,7 @@ def algorithmic_bytes(cfg):
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -167,7 +172,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+    return 3350.0, "fallback 3.35 TB/s (H100 SXM data sheet HBM3 bandwidth)"
 
 
 # =============================================================================
@@ -279,7 +284,7 @@ def workload_config(args, note=None):
                      f"{N_FRAMES} frames",
          "rays_per_step": args.rays, "ray_batch": args.ray_batch, "n_levels_hash": args.levels,
          "parallelism": f"ray-sharded dp{args.gpus}", "streams": getattr(args, "streams", 1), "loss": getattr(args, "loss", None), "pipeline": getattr(args, "pipeline", None), "mlp": getattr(args, "mlp", None),
-         "l2": "inputs larger than L2: fp16/fp32 working set > 126 MB plus > 1 GB of saved activations streamed per step"}
+         "l2": "inputs larger than L2: fp16/fp32 working set > 50 MB (the H100 L2) plus > 1 GB of saved activations streamed per step"}
     if note:
         c["note"] = note
     return c
@@ -321,8 +326,8 @@ def red_counts(cfg, rays=None):
 
 
 def micro_peaks():
-    """Measured ceilings of the units that actually bind the kernels (profiles/r02_micro_peaks.json, from
-    scripts/micro/{gather,red}_bench.cu on a B200 of this pool): divergent L2-resident sector gathers, RED.128 lane-ops."""
+    """Measured ceilings of the units that actually bind the kernels (profiles/r02_micro_peaks.json, written by
+    scripts/micro/{gather,red}_bench.cu when measured): divergent L2-resident sector gathers, RED.128 lane-ops."""
     p = os.path.join(ROOT, "profiles", "r02_micro_peaks.json")
     if os.path.exists(p):
         return json.load(open(p))
@@ -378,6 +383,21 @@ def gpu_eager_baseline(levels, n_rays, dev):
         return res
     except Exception as e:          # a baseline leg must never take the bench line down
         return {"value": None, "unit": "rays/s", "error": repr(e)[:200]}
+
+
+def dump_outputs(out_dir, model, last):
+    """What the last timed step returned to its caller, as float32 .npy files (at most a few MB at the default sizes)."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"depth": last["rays"][:, 0], "image": last["rays"][:, 1:3]}
+    if "loss" in last:
+        arrays["loss"] = last["loss"].reshape(1)
+        arrays["sigma_net_params"] = model.sigma_net.params.detach()
+        hs = model.hash_encoder.hash_static.params.detach().reshape(-1)
+        sel = torch.from_numpy(np.random.default_rng(0).choice(hs.numel(), min(hs.numel(), 1 << 20), replace=False)).to(hs.device)
+        arrays["hash_static_params_sample"] = hs[sel]
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a.float().cpu().numpy())
+    log(f"outputs of the last timed step -> {out_dir}: " + ", ".join(f"{k} {tuple(v.shape)}" for k, v in arrays.items()))
 
 
 def run_b200(args):
@@ -446,7 +466,11 @@ def run_b200(args):
     n_streams = max(1, min(args.streams, n_chunks))
     side = [torch.cuda.Stream(device=dev) for _ in range(n_streams)] if n_streams > 1 else []
 
-    def chunk(h, ro_d, rd_d, t, e2e, last):
+    # --dump-outputs: the step index whose results are kept (the last timed step); no other step does extra work
+    dump = {"at": args.warmup + args.steps - 1 if args.dump_outputs is not None else None}
+    last_out = {}
+
+    def chunk(h, ro_d, rd_d, t, e2e, last, keep=False):
         out = model.render(ro_d[None, h:h + rb], rd_d[None, h:h + rb], t, staged=False, num_steps=S_STEPS,
                            perturb=True, ray_offset=ray_off0 + h)
         # the reference's main loss (runner.py:193-213: L1 depth, label-smoothed ray-drop MSE, intensity MSE, defaults of
@@ -460,12 +484,13 @@ def run_b200(args):
         else:
             loss.backward()
         res = None
-        if e2e:
+        if e2e or keep:
             res = torch.cat([out["depth_lidar"].detach().view(-1, 1), out["image_lidar"].detach().view(-1, 2)], 1)
         return loss.detach(), res
 
     def train_step(i, e2e, streams=True):
         ro_d, rd_d, t = inputs(i, e2e)
+        keep = i == dump["at"]
         opt.zero_grad(set_to_none=True)
         main = torch.cuda.current_stream()
         parts, outs = [], []
@@ -475,7 +500,7 @@ def run_b200(args):
                 st.wait_stream(main)
             for c, h in enumerate(range(0, n_rays, rb)):
                 with torch.cuda.stream(side[c % n_streams]):
-                    l, r = chunk(h, ro_d, rd_d, t, e2e, False)
+                    l, r = chunk(h, ro_d, rd_d, t, e2e, False, keep)
                     parts.append(l)
                     outs.append(r)
             for st in side:
@@ -484,7 +509,7 @@ def run_b200(args):
                 x.record_stream(main)
         else:
             for h in range(0, n_rays, rb):
-                l, r = chunk(h, ro_d, rd_d, t, e2e, h + rb >= n_rays)
+                l, r = chunk(h, ro_d, rd_d, t, e2e, h + rb >= n_rays, keep)
                 parts.append(l)
                 outs.append(r)
         tot = torch.stack(parts).sum()
@@ -497,6 +522,8 @@ def run_b200(args):
             train_step.adam_events.append(ev)
         else:
             opt.step()
+        if keep:
+            last_out.update(rays=torch.cat(outs, 0), loss=tot)
         if e2e:
             host_out.copy_(torch.cat(outs, 0), non_blocking=True)
             return float(tot)            # device->host read of the step's loss (sync)
@@ -508,6 +535,8 @@ def run_b200(args):
         ro_d, rd_d, t = inputs(i, e2e)
         with torch.no_grad():
             out = model.render(ro_d[None], rd_d[None], t, staged=False, num_steps=S_STEPS, perturb=False, ray_offset=ray_off0)
+        if i == dump["at"]:
+            last_out.update(rays=torch.cat([out["depth_lidar"].view(-1, 1), out["image_lidar"].view(-1, 2)], 1))
         if e2e:
             host_out[:, 0:1].copy_(out["depth_lidar"].view(-1, 1), non_blocking=True)
             host_out[:, 1:3].copy_(out["image_lidar"].view(-1, 2), non_blocking=True)
@@ -552,6 +581,10 @@ def run_b200(args):
     ms, launches = timed(False, args.steps, args.warmup)
     clocks = sampler.stop() if rank == 0 else {}
     log(f"timed: {ms / args.steps:.2f} ms/step")
+    if dump["at"] is not None:
+        dump["at"] = None
+        if rank == 0:
+            dump_outputs(args.dump_outputs, model, last_out)
     step(0, True)                                  # warm the e2e path (pinned copies)
     ms_e2e, _ = timed(True, args.steps, args.warmup)
     peak_mem = torch.cuda.max_memory_allocated() / 1e9
@@ -660,7 +693,7 @@ def run_b200(args):
         "metric": metric, "value": value, "unit": "rays/s",
         "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms / args.steps,
         "higher_is_better": True, "scaling": "strong" if strong else "weak", "vs_baseline": None,
-        "dtype": ("fp16 tables + fp16 MLP weights (tcgen05, hi/lo fp16 activations, fp32 accumulate)" if args.mlp == "fp16"
+        "dtype": ("fp16 tables + fp16 MLP weights (wgmma, hi/lo fp16 activations, fp32 accumulate)" if args.mlp == "fp16"
                   else "fp16 tables, fp32 MLPs") + "; fp32 planes, compositing and gradients", "data": "synthetic",
         "config": cfgd,
         "e2e": {"value": total_rays / (ms_e2e * 1e-3), "unit": "rays/s", "h2d_bytes_per_step": n_rays * 6 * 4,

@@ -1,5 +1,5 @@
 /*
- * lidar4d_b200.h - C-ABI of the B200 (sm_100a) LiDAR4D hot-path library
+ * lidar4d_b200.h - C-ABI of the H100 (sm_90a) LiDAR4D hot-path library
  * (liblidar4d_b200.so).  Plain C: pointers, sizes, POD structs; no torch / ATen
  * types cross this boundary.
  *
@@ -85,7 +85,7 @@ typedef struct L4DConfig {
   float    far_lidar;
   float    density_scale;
   uint32_t mlp_fp16;             /* 1: MLP weights are consumed as fp16-rounded working copies (as tcnn's half
-                                    params) and the dense kernels run on tcgen05 tensor cores; 0: fp32 FMA */
+                                    params) and the dense kernels run on wgmma tensor cores; 0: fp32 FMA */
   uint32_t reserved;
 } L4DConfig;
 
@@ -279,7 +279,7 @@ unsigned long long l4d_launch_count(void);
 int    l4d_profile_start(void);
 int    l4d_profile_stop(const char** names, float* ms, int cap);
 
-/* tcgen05/TMEM self-test of the MLP engine's building blocks: C[128,N] = A[128,K] * B[N,K]^T,
+/* wgmma self-test of the MLP engine's building blocks: C[128,N] = A[128,K] * B[N,K]^T,
  * fp16 operands, fp32 accumulate (N%16==0 in [16,256], K%16==0 in [16,512]). */
 int    l4d_tc_selftest(const void* A_half, const void* B_half, float* C, uint32_t N, uint32_t K, void* stream);
 /* same with operands pre-arranged in the engine's tile format, M in {64,128}, K-major or MN-major operands

@@ -1,4 +1,4 @@
-"""lidar4d_b200 - B200-native (sm_100a) implementation of the LiDAR4D per-ray
+"""lidar4d_b200 - H100-native (sm_90a) implementation of the LiDAR4D per-ray
 volume-rendering hot path behind the reference's LiDAR4D nn.Module API.
 
 `from lidar4d_b200 import LiDAR4D` gives the drop-in module; it loads

@@ -234,7 +234,7 @@ def load_library():
     if not os.path.exists(path):
         raise RuntimeError(
             f"{path} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a).  lidar4d_b200 has no CPU fallback.")
+            "(nvcc, sm_90a).  lidar4d_b200 has no CPU fallback.")
     lib = C.CDLL(path)
     declare(lib)
     if lib.l4d_abi_version() != ABI_VERSION:

@@ -394,8 +394,8 @@ struct DfeatFromPlane {
 #define L4D_SC_ALL 7
 // L4D_SCATTER_INTERLEAVE (A/B knob, default off): issue the dynamic-hash REDs in slices BETWEEN the plane sinks instead of back to
 // back at the end (1 = one slice per time-plane query, 2 = one per plane sink).  The idea - the sinks are issue / shuffle work,
-// the REDs L2-atomic work, let them overlap inside a warp - measured SLOWER on the B200: k_bwd_scatter 19.4 ms (0) vs 23.3 ms (2)
-// per 16,384 rays at L = 16 (profiles/r02_v8_ab_contract.txt); the warps of an SM already sit in different phases.
+// the REDs L2-atomic work, let them overlap inside a warp - not measured on the H100; off because the warps of an SM already
+// sit in different phases.
 #ifndef L4D_SCATTER_INTERLEAVE
 #define L4D_SCATTER_INTERLEAVE 0
 #endif

@@ -6,13 +6,13 @@
 //   idx1[b,j]  = the smallest k attaining it        (strict '<' while scanning k upwards, '>' across 512-chunks)
 //   and the same with the roles of the clouds swapped; backward: d dist / d point = 2 (p1 - p2) on both ends.
 //
-// B200 design.  The reference launches a fixed 32 x 16 grid whose x-dimension strides over the batch: with b = 1
+// Design.  The reference launches a fixed 32 x 16 grid whose x-dimension strides over the batch: with b = 1
 // (every call in runner.py:216-251) 16 CTAs are busy.  Here the query cloud is cut into blocks of 256 threads x Q
-// queries and, when that does not fill 148 SMs twice, the target cloud is split across gridDim.y as well; partial
+// queries and, when that does not fill the SMs twice, the target cloud is split across gridDim.y as well; partial
 // results meet in a 64-bit atomicMin on (distance bits << 32 | index): for non-negative floats the integer order is
 // the float order and ties resolve to the smaller index, i.e. exactly the reference's rule.  Targets are staged in
-// shared memory as coordinate-wise pairs of consecutive points, so a broadcast LDS.64 is already a packed fp32x2
-// operand: the distance of one query to two targets costs 3 FADD2 + 1 FMUL2 + 2 FFMA2 (sm_100 packed fp32), four
+// shared memory as coordinate-wise pairs of consecutive points, so one broadcast LDS.64 per coordinate serves two
+// targets: the distance of one query to two targets costs 6 FADD + 2 FMUL + 4 FFMA, four
 // targets are screened with one min/compare against the running best, and the (rare) update is resolved in scan
 // order - FP32-pipe bound, no tensor cores (K = 3 is not a GEMM, and the reference's rounding is part of the result).
 // (included at the end of l4d_kernels.cu: one translation unit, one shared library)
@@ -27,13 +27,14 @@ constexpr int CH_TILE = 2048;   // target points per shared-memory tile (24 KB a
 __device__ __forceinline__ unsigned long long pack_key(float d, uint32_t idx) {
   return ((unsigned long long)__float_as_uint(d) << 32) | (unsigned long long)idx;
 }
-// packed fp32x2 arithmetic (sm_100: FADD2 / FMUL2 / FFMA2, IEEE round-to-nearest per lane)
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pk2(float a, float b) { f32x2 r; asm("mov.b64 %0, {%1,%2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void upk2(f32x2 v, float& a, float& b) { asm("mov.b64 {%0,%1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ f32x2 sub2(f32x2 a, f32x2 b) { f32x2 r; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { f32x2 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { f32x2 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
+// coordinate-wise pairs of fp32 (two targets per operand), IEEE round-to-nearest per lane: sm_90 has no packed fp32
+// instructions, so each pair operation is two FADD / FMUL / FFMA with the rounding of the packed form
+typedef float2 f32x2;
+__device__ __forceinline__ f32x2 pk2(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ void upk2(f32x2 v, float& a, float& b) { a = v.x; b = v.y; }
+__device__ __forceinline__ f32x2 sub2(f32x2 a, f32x2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
+__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
 
 // two consecutive targets (k, k+1), coordinate-wise: one LDS.64 per coordinate yields a packed operand
 struct __align__(8) TargetPair { float2 x, y, z; };
@@ -148,7 +149,7 @@ __global__ void k_chamfer_grad(uint32_t nq, const float* __restrict__ q, uint32_
 }
 
 // target splits so that every SM gets about eight CTAs (four are resident at a time): with only two per SM the last,
-// partial wave cost 12 % (ncu: 392 CTAs on 148 SMs, 28 % warps active)
+// partial wave leaves most of the SMs idle
 static uint32_t splits_for(uint32_t b, uint32_t nq, uint32_t nt) {
   const uint32_t qblocks = (nq + CH_NT * CH_Q - 1) / (CH_NT * CH_Q);
   const uint32_t want = 8u * (uint32_t)sm_count();

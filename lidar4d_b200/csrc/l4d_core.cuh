@@ -1,5 +1,5 @@
 // l4d_core.cuh - per-sample arithmetic of the LiDAR4D hot path, written once as
-// __host__ __device__ code.  The sm_100a kernels (l4d_kernels.cu) call these per
+// __host__ __device__ code.  The sm_90a kernels (l4d_kernels.cu) call these per
 // thread (thread == sample); tests/hostsim compiles the same functions for the
 // host so the math can be checked against the oracle without a GPU.  The host
 // build is TEST infrastructure only - the product has no CPU path.
@@ -78,7 +78,7 @@ struct DevModel {
   const float *sig_w1t, *sig_w2t, *sig_w2;
   const float *att_w1t[2], *att_w2t[2], *att_w2[2], *att_w3[2];   // net 0 = raydrop, 1 = intensity
   const float *flo_w0t, *flo_w1t, *flo_w1, *flo_w2t, *flo_w2;
-  // fp16 copies in the tcgen05 K-major interleaved layout [k/8][row n][8 halves] (element (n,k) = W[n][k])
+  // fp16 copies in the wgmma K-major interleaved layout [k/8][row n][8 halves] (element (n,k) = W[n][k])
   const __half *tc_sig_w1, *tc_sig_w2, *tc_att_w1g, *tc_att_w2[2], *tc_att_w1g_net[2];
   const __half *tc_flo_w0, *tc_flo_w1, *tc_flo_w2;     // [2][64][8], [8][64][8], [8][16][8] (rows 6..15 zero)
   uint32_t mlp_fp16;
@@ -358,12 +358,12 @@ L4D_HD float l4d_contract_entry(uint4 rec, const L4DTimeQuery& q, uint32_t n_sli
   return ((q.basis[0] * fl[0] + q.basis[1] * fl[1]) + q.basis[2] * fl[2]) + q.basis[3] * fl[3];
 }
 // one level of one contracted dynamic table at (x,y): bilinear blend of four fp32 entries.
-// L4D_CON_GATHER (A/B, measured on the B200, ms of k_fwd_gather per 16,384 rays at L = 16; pair records: 21.3):
+// L4D_CON_GATHER (A/B knob; timings not measured on the H100):
 //   0  one 16-byte load of the aligned quad of entries that holds the first x-corner (the second x-corner is in the same
-//      quad three times out of four) + a conditional 4-byte load otherwise: 2.5 instead of 4 sector requests per level, but
-//      a divergent branch per row - 25.8 ms: the loads of a level no longer overlap
-//   1  four independent 4-byte loads (no branch, no selects) - 17.7 ms (16.4 ms at 8 CTAs/SM): the default
-//   2  the quad load + an unconditional 4-byte load of the second x-corner - 23.5 ms
+//      quad three times out of four) + a conditional 4-byte load otherwise: fewer sector requests per level, but a
+//      divergent branch per row, so the loads of a level no longer overlap
+//   1  four independent 4-byte loads (no branch, no selects): the default
+//   2  the quad load + an unconditional 4-byte load of the second x-corner
 #ifndef L4D_CON_GATHER
 #define L4D_CON_GATHER 1
 #endif
@@ -600,7 +600,7 @@ L4D_HD RaySampling l4d_make_sampling(float near_, float far_, uint32_t S, uint32
 // torch.linspace(0,1,S) as the CUDA kernel computes it, then near + span*lin (+ jitter)
 L4D_HD float l4d_z(const RaySampling& r, uint64_t ray_global, uint32_t j) {
   // ATen's linspace kernel (RangeFactories.cu): `start + step*i` below the midpoint, `end - step*(S-1-i)` above it; nvcc
-  // contracts the latter into ONE fma (measured on the B200: tests/golden/cuda_linspace.npz), the former is exact either way
+  // contracts the latter into ONE fma (tests/golden/cuda_linspace.npz), the former is exact either way
   float lin = (j < r.S / 2) ? L4D_MUL(r.lin_step, (float)j)
                             : fmaf(-r.lin_step, (float)(r.S - 1 - j), 1.0f);
   float z = L4D_ADD(r.near_, L4D_MUL(r.span, lin));

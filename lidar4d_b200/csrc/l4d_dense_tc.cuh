@@ -1,13 +1,14 @@
-// l4d_dense_tc.cuh - tensor-core (tcgen05 / TMEM) versions of the dense kernels of the split
-// pipeline.  Requires mlp_fp16 (MLP weights are fp16 working copies, as tiny-cuda-nn keeps them).
+// l4d_dense_tc.cuh - tensor-core (wgmma) versions of the dense kernels of the split pipeline.
+// Requires mlp_fp16 (MLP weights are fp16 working copies, as tiny-cuda-nn keeps them).
 //
-// Tile = 128 samples = the 128 TMEM lanes = the 128 threads of the CTA (thread == sample == row).
+// Tile = 128 samples; in the epilogues thread (threadIdx.x % 128) owns sample row.
 // Operands live in shared memory as fp16 in the K-major interleaved layout of l4d_tc.cuh
 // ([k/8][row][8 halves], 16-byte chunks).  Activations are carried as hi + lo fp16 pairs
 // (x = hi + lo to ~2^-22 relative), i.e. every product with an fp16 weight is exact and the fp32
-// TMEM accumulation reproduces the fp32-FMA kernels to ~1e-6: the 1e-4 parity bar holds on the
-// tensor-core path too.  One elected thread issues the MMAs; completion is tracked with one
-// mbarrier (tcgen05.commit), accumulators are read back with tcgen05.ld 32x32b (lane == thread).
+// accumulation reproduces the fp32-FMA kernels to ~1e-6: the 1e-4 parity bar holds on the
+// tensor-core path too.  Every warpgroup issues the wgmma of its 64-row block; activation products
+// go through the fp32 staging tile (one row per thread), weight gradients are flushed with fp32
+// atomics straight from the accumulator registers.
 #pragma once
 #include "l4d_core.cuh"
 #include "l4d_tc.cuh"
@@ -36,37 +37,45 @@ __device__ __forceinline__ void tile_put8(unsigned char* hi, unsigned char* lo, 
   *reinterpret_cast<uint4*>(tile_chunk(lo, r, c)) = pack8_half(res);
 }
 
-// D[128 x N] (+)= A * B^T over n_chunks 16-byte k-chunks (n_chunks even): A chunks at a_saddr + c*2048,
-// B (N rows) chunks at b_saddr + c*N*16.  Issued by ONE thread.
-__device__ __forceinline__ void mma_chunks(uint32_t d_tmem, uint32_t a_saddr, uint32_t b_saddr, uint32_t N, int n_chunks,
-                                           bool accumulate) {
-  const uint32_t idesc = idesc_f16(128, N);
-  for (int c = 0; c < n_chunks; c += 2) {
-    const uint64_t da = smem_desc(a_saddr + (uint32_t)c * 2048u, 2048u, 128u);
-    const uint64_t db = smem_desc(b_saddr + (uint32_t)c * N * 16u, N * 16u, 128u);
-    umma_f16(d_tmem, da, db, idesc, (accumulate || c > 0) ? 1u : 0u);
-  }
+// all threads: make generic-proxy tile writes visible to the tensor cores, then barrier
+__device__ __forceinline__ void publish() {
+  fence_proxy_async();
+  __syncthreads();
 }
 
-struct MmaSync {
-  uint64_t* bar;
-  uint32_t phase;
-  // all threads: make generic-proxy tile writes visible, then barrier
-  __device__ __forceinline__ void publish() {
-    fence_proxy_async();
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
+// The products below are called by every thread of the CTA; the warpgroups split the two 64-row blocks of a
+// 128-sample product.  A thread may read the staging tile only after the __syncthreads() that follows.
+//
+// D[128 x N] = (Ah + Al) * B^T over n_chunks 16-byte k-chunks (n_chunks even): A = 128-row tiles (chunk stride 2048),
+// B = K-major [k/8][b_rows][8] (b points at its first used row) -> staging columns [c0, c0 + N)
+template <int N>
+__device__ __forceinline__ void mma_rows(float* S, int c0, uint32_t a_hi, uint32_t a_lo, uint32_t b, uint32_t b_rows, int n_chunks) {
+  for (int mb = threadIdx.x >> 7; mb < 2; mb += blockDim.x >> 7) {
+    const Opnd a{{a_hi + (uint32_t)mb * 1024u, a_lo + (uint32_t)mb * 1024u, 0u}, 4096u, 2048u, 128u};
+    const Opnd w{{b, b, 0u}, 2u * b_rows * 16u, b_rows * 16u, 128u};
+    float d[N / 2];
+    wg_gemm<N, 0, 0>(d, a, w, 2, n_chunks / 2);
+    acc_store<N>(S, d, 64 * mb, c0);
   }
-  // issuing thread: after its MMAs
-  __device__ __forceinline__ void commit() { umma_commit(bar); }
-  // all threads: wait for the committed MMAs
-  __device__ __forceinline__ void wait() {
-    mbar_wait(bar, phase);
-    phase ^= 1u;
-    tc_fence_after();
+}
+// D[128 x N] = (Ah + Al) * W: W stored [k_in/8][w_rows][8] (forward layout) and read as B(n = k_in, k = row), i.e.
+// MN-major; w points at the chunk of the first k_in column used.  f(row, col, v[col], v[col + 1]) per element pair.
+template <int N, class F>
+__device__ __forceinline__ void mma_prop_frag(uint32_t a_hi, uint32_t a_lo, int n_chunks, uint32_t w, uint32_t w_rows, F&& f) {
+  for (int mb = threadIdx.x >> 7; mb < 2; mb += blockDim.x >> 7) {
+    const Opnd a{{a_hi + (uint32_t)mb * 1024u, a_lo + (uint32_t)mb * 1024u, 0u}, 4096u, 2048u, 128u};
+    const Opnd b{{w, w, 0u}, 256u, 128u, w_rows * 16u};
+    float d[N / 2];
+    wg_gemm<N, 0, 1>(d, a, b, 2, n_chunks / 2);
+    frag_foreach<N>(d, [&](int r, int c, float x, float y) { f(64 * mb + r, c, x, y); });
   }
-};
+}
+template <int N>
+__device__ __forceinline__ void mma_prop(float* S, int c0, uint32_t a_hi, uint32_t a_lo, int n_chunks, uint32_t w, uint32_t w_rows) {
+  mma_prop_frag<N>(a_hi, a_lo, n_chunks, w, w_rows, [&](int r, int c, float x, float y) {
+    *reinterpret_cast<float2*>(S + acc_idx(r, c0 + c)) = make_float2(x, y);
+  });
+}
 
 }  // namespace l4dtc
 
@@ -77,6 +86,7 @@ struct DenseFwdSmem {
   uint32_t hh, hl;                  // 64-wide hidden tile
   uint32_t gh, gl;                  // 16-wide tile (geo)
   uint32_t misc;                    // enc[80] cdir[128] w[32] floats
+  uint32_t acc;                     // fp32 staging tile
   uint32_t total;
 };
 __host__ __device__ inline DenseFwdSmem dense_fwd_smem(uint32_t in_pad) {
@@ -90,6 +100,7 @@ __host__ __device__ inline DenseFwdSmem dense_fwd_smem(uint32_t in_pad) {
   L.hh = take(64 * 128 * 2); L.hl = take(64 * 128 * 2);
   L.gh = take(16 * 128 * 2); L.gl = take(16 * 128 * 2);
   L.misc = take((80 + 128 + 32) * 4);
+  L.acc = take(l4dtc::acc_tile_bytes());
   L.total = o;
   return L;
 }
@@ -97,17 +108,16 @@ __host__ __device__ inline DenseFwdSmem dense_fwd_smem(uint32_t in_pad) {
 // =============================================================================================
 // backward 1/3 on tensor cores.
 //
-// Every GEMM of the dense backward runs as tcgen05 MMAs on 128-sample tiles:
+// Every GEMM of the dense backward runs as wgmma on 128-sample tiles:
 //   forward recompute   Y = A * W^T            A K-major tile (hi+lo), W K-major weights
 //   delta propagation   dA = dY * W            dY K-major tile (hi+lo), W read as an MN-major operand
 //   weight gradients    dW^T = A^T * dY        both sample-major tiles read as MN-major operands
 //                                              (3 terms: Ah*dh + Al*dh + Ah*dl)
 // Gradient tiles are stored as fp16 hi/lo pairs after a per-tile power-of-two scale (block amax), so
 // loss-scaled or tiny upstream gradients neither overflow nor flush; the scale is undone when the
-// fp32 accumulators are read back.  Weight-gradient accumulators are flushed from TMEM with fp32
+// fp32 accumulators are read back.  Weight-gradient accumulators are flushed from the registers with fp32
 // atomics once per tile (same count as the FMA kernel's tile_outer_accum).
-// TMEM columns:  [0,64) work A   [64,128) work B   [128,144) O / dG   [144,160) dW2s^T  [160,176) dW1g
-//                [176,184) dw3   [192,256) dW2a^T / dW1^T(a)   [256,256+in_pad) dX   [448,512) dW1^T(b)
+// Shared memory at sigma_in_pad = 176 (L = 16): 226 KB, within the 227 KB an sm_90 CTA may use; one CTA per SM.
 // =============================================================================================
 struct DenseBwdSmem {
   uint32_t w1, w2, wa1[2], wa2[2];
@@ -115,6 +125,7 @@ struct DenseBwdSmem {
   uint32_t RH;           // 32 KB: sigma hidden hi|lo, later its delta
   uint32_t g16, do16, do8;   // small tiles, hi|lo
   uint32_t misc;
+  uint32_t acc;          // 32 KB fp32 staging tile
   uint32_t total;
 };
 __host__ __device__ inline DenseBwdSmem dense_bwd_smem(uint32_t in_pad) {
@@ -127,32 +138,23 @@ __host__ __device__ inline DenseBwdSmem dense_bwd_smem(uint32_t in_pad) {
   L.R = take(96 * 1024); L.RH = take(32 * 1024);
   L.g16 = take(2 * 4096); L.do16 = take(2 * 4096); L.do8 = take(2 * 2048);
   L.misc = take((80 + 128 + 128 + 128 + 32 + 64) * 4);
+  L.acc = take(l4dtc::acc_tile_bytes());
   L.total = o;
   return L;
 }
 
 namespace l4dtc {
-// dW^T[M x N] (+)= A^T * B over the 128 samples of two sample-major tiles read as MN-major operands;
-// a_addr / b_addr = shared address of the first 16-byte feature chunk of the operand.
-__device__ __forceinline__ void mma_tt(uint32_t d_tmem, uint32_t a_addr, uint32_t M, uint32_t b_addr, uint32_t N, bool accumulate) {
-  const uint32_t idesc = idesc_f16(M, N, 1u, 1u);
-  for (uint32_t k = 0; k < 8; ++k) {
-    const uint64_t da = smem_desc(a_addr + k * 256u, 128u, 2048u);
-    const uint64_t db = smem_desc(b_addr + k * 256u, 128u, 2048u);
-    umma_f16(d_tmem, da, db, idesc, (accumulate || k > 0) ? 1u : 0u);
-  }
+// dW^T[64 x N] = Ah^T * Bh + Al^T * Bh + Ah^T * Bl over the 128 samples of sample-major tiles read as MN-major operands;
+// a / b = shared address of the first 16-byte feature chunk used.  Warpgroup-wide; f(row, col, v[col], v[col + 1]).
+template <int N, class F>
+__device__ __forceinline__ void mma_tt(uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, F&& f) {
+  const Opnd a{{a_hi, a_lo, a_hi}, 256u, 128u, 2048u};
+  const Opnd b{{b_hi, b_hi, b_lo}, 256u, 128u, 2048u};
+  float d[N / 2];
+  wg_gemm<N, 1, 1>(d, a, b, 3, 8);
+  frag_foreach<N>(d, f);
 }
-// dA[128 x N] (+)= dY * W: dY K-major tile with n_chunks 16-byte chunks, W stored [k_in/8][rows][8] (forward layout),
-// read as B(n = k_in, k = row): MN-major with SBO = rows*16
-__device__ __forceinline__ void mma_prop(uint32_t d_tmem, uint32_t a_addr, int n_chunks, uint32_t w_addr, uint32_t w_rows,
-                                         uint32_t N, bool accumulate) {
-  const uint32_t idesc = idesc_f16(128, N, 0u, 1u);
-  for (int c = 0; c < n_chunks; c += 2) {
-    const uint64_t da = smem_desc(a_addr + (uint32_t)c * 2048u, 2048u, 128u);
-    const uint64_t db = smem_desc(w_addr + (uint32_t)(c / 2) * 256u, 128u, w_rows * 16u);
-    umma_f16(d_tmem, da, db, idesc, (accumulate || c > 0) ? 1u : 0u);
-  }
-}
+__device__ __forceinline__ void red2(float* p, float a, float b) { atomicAdd(reinterpret_cast<float2*>(p), make_float2(a, b)); }
 __device__ __forceinline__ float block_amax128(float v, float* s_w) {
   v = fabsf(v);
 #pragma unroll
@@ -236,9 +238,8 @@ __device__ __forceinline__ float block_amax256(float v, float* s_w) {
 
 // -------------------------------------------------------------------------------------------
 // forward 2/2 on tensor cores: sigma MLP, compositing, attribute heads.  One CTA per ray, 256 threads: two threads per
-// row (sample) split the columns of every epilogue; in the attribute phase thread half h owns head h.
-// TMEM columns: [0,64) sigma hidden / attribute layer-2 net0, [64,128) attribute layer-2 net1,
-//               [128,144) sigma output, [256,384) attribute layer-1 (both heads)
+// row (sample) split the columns of every epilogue; in the attribute phase thread half h owns head h, and the heads'
+// products pass through the 64-column staging tile one after the other.
 // -------------------------------------------------------------------------------------------
 namespace l4dtc {
 // sum over the 128 rows of one thread half (warps 0-3 / 4-7) of a 256-thread CTA; every thread of the half gets it
@@ -256,22 +257,21 @@ __device__ __forceinline__ float half_sum(float v, float* s_w) {
 
 __global__ void __launch_bounds__(256) k_fwd_dense_tc(const __grid_constant__ SplitArgs A) {
   using namespace l4dtc;
-  extern __shared__ __align__(1024) unsigned char dsm[];
-  __shared__ __align__(8) uint64_t s_bar, s_xbar;
-  __shared__ uint32_t s_tmem;
+  extern __shared__ __align__(128) unsigned char dsm[];
+  __shared__ __align__(8) uint64_t s_xbar;
   const DevModel& M = A.M;
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int row = tid & 127, half = tid >> 7, wq = warp & 3;
+  const int tid = threadIdx.x;
+  const int row = tid & 127, half = tid >> 7;
   const uint32_t in_pad = M.sigma_in_pad;
   const DenseFwdSmem L = dense_fwd_smem(in_pad);
   unsigned char *xh = dsm + L.xh, *xl = dsm + L.xl, *hh = dsm + L.hh, *hl = dsm + L.hl, *gh = dsm + L.gh, *gl = dsm + L.gl;
   float* s_enc = reinterpret_cast<float*>(dsm + L.misc);
   float* s_cdir = s_enc + 80;
   float* s_w = s_cdir + 128;
+  float* S = reinterpret_cast<float*>(dsm + L.acc);
   const uint32_t sb = smem_u32(dsm);
 
-  if (tid == 0) { mbar_init(&s_bar, 1); mbar_init(&s_xbar, 1); fence_mbar_init(); }
-  if (warp == 0) tmem_alloc(&s_tmem, 512);
+  if (tid == 0) { mbar_init(&s_xbar, 1); fence_mbar_init(); }
   // weights -> shared memory (already in operand layout in global memory)
   {
     auto cp = [&](uint32_t off, const __half* src, uint32_t bytes) {
@@ -284,12 +284,9 @@ __global__ void __launch_bounds__(256) k_fwd_dense_tc(const __grid_constant__ Sp
     cp(L.wa2[0], M.tc_att_w2[0], 64 * 64 * 2);
     cp(L.wa2[1], M.tc_att_w2[1], 64 * 64 * 2);
   }
-  MmaSync ms{&s_bar, 0u};
-  ms.publish();
-  const uint32_t tm = s_tmem;
-  const uint32_t tlane = tm + ((uint32_t)(wq * 32) << 16);
+  publish();
   const RaySampling rs = l4d_make_sampling(M.near_lidar, M.far_lidar, A.S, A.perturb, A.seed);
-  const uint32_t S = A.S;
+  const uint32_t n_steps = A.S;
   const int n_xchunks = (int)in_pad / 8;
   // feature tiles arrive as fp16 hi|lo operand tiles (written by k_fwd_gather) with one bulk copy per half; the copy of
   // the next tile is issued as soon as the last MMA that reads the X buffer has completed
@@ -329,45 +326,37 @@ __global__ void __launch_bounds__(256) k_fwd_dense_tc(const __grid_constant__ Sp
     // per-thread partial sums over this thread's row: half 0 carries depth, weight sum and head 0, half 1 carries head 1
     float carry = 1.f, pd = 0.f, pa = 0.f, pw = 0.f;
     const uint64_t rg = A.ray_offset + ray;
-    for (uint32_t j0 = 0; j0 < S; j0 += 128) {
+    for (uint32_t j0 = 0; j0 < n_steps; j0 += 128) {
       const uint32_t j = j0 + row;
-      const bool valid = j < S;
-      const size_t p = (size_t)ray * S + (valid ? j : 0);
+      const bool valid = j < n_steps;
+      const size_t p = (size_t)ray * n_steps + (valid ? j : 0);
       if (tid == 0 && A.train) A.sv.tstart[(size_t)ray * n_tiles + (j0 >> 7)] = carry;     // the backward starts every tile from here
       mbar_wait(&s_xbar, xphase);      // this tile's features have landed
       xphase ^= 1u;
-      ms.publish();
-      if (tid == 0) {
-        mma_chunks(tm + 0, sb + L.xh, sb + L.w1, 64, n_xchunks, false);
-        mma_chunks(tm + 0, sb + L.xl, sb + L.w1, 64, n_xchunks, true);
-        ms.commit();
-      }
-      ms.wait();
+      publish();
+      mma_rows<64>(S, 0, sb + L.xh, sb + L.xl, sb + L.w1, 64, n_xchunks);
+      __syncthreads();
       // ---- hidden = relu(.) -> hi/lo tile (each half its 32 columns) ----
 #pragma unroll
       for (int qq = 0; qq < 2; ++qq) {
         const int q = 2 * half + qq;
         float v[16];
-        tmem_ld16(tlane + (uint32_t)(q * 16), v);
+        acc_ld16(S, q * 16, v);
 #pragma unroll
         for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i], 0.f);
         tile_put8(hh, hl, row, 2 * q, v);
         tile_put8(hh, hl, row, 2 * q + 1, v + 8);
       }
-      ms.publish();
-      if (tid == 0) {
-        mma_chunks(tm + 128, sb + L.hh, sb + L.w2, 16, 8, false);
-        mma_chunks(tm + 128, sb + L.hl, sb + L.w2, 16, 8, true);
-        ms.commit();
-      }
-      ms.wait();
+      publish();
+      mma_rows<16>(S, 0, sb + L.hh, sb + L.hl, sb + L.w2, 16, 8);
+      __syncthreads();
       float out[16];
-      tmem_ld16(tlane + 128u, out);
+      acc_ld16(S, 0, out);
       float zj = 0.f, alpha = 0.f, sigma = 0.f;
       if (valid) {
         sigma = expf(out[0]);
         zj = l4d_z(rs, rg, j);
-        const float delta = (j + 1 < S) ? (l4d_z(rs, rg, j + 1) - zj) : rs.sample_dist;
+        const float delta = (j + 1 < n_steps) ? (l4d_z(rs, rg, j + 1) - zj) : rs.sample_dist;
         alpha = l4d_alpha(M, delta, sigma);
       }
       const float vv = valid ? (1.0f - alpha) + 1e-15f : 1.f;
@@ -390,42 +379,42 @@ __global__ void __launch_bounds__(256) k_fwd_dense_tc(const __grid_constant__ Sp
           }
           tile_put8(gh, gl, row, half, g8);
         }
-        ms.publish();
-        if (tid == 0) {
-          mma_chunks(tm + 256, sb + L.gh, sb + L.wa1, 128, 2, false);
-          mma_chunks(tm + 256, sb + L.gl, sb + L.wa1, 128, 2, true);
-          ms.commit();
-        }
-        ms.wait();
+        publish();
+#pragma unroll 1
+        for (int net = 0; net < 2; ++net) {    // 128 columns: net0 hidden | net1 hidden -> chunks 0..15 of the x tile
+          mma_rows<64>(S, 0, sb + L.gh, sb + L.gl, sb + L.wa1 + (uint32_t)net * 64u * 16u, 128, 2);
+          __syncthreads();
+          if (half == net) {
 #pragma unroll
-        for (int qq = 0; qq < 4; ++qq) {     // 128 columns: net0 hidden | net1 hidden -> chunks 0..15 of the x tile
-          const int q = 4 * half + qq;
-          float v[16];
-          tmem_ld16(tlane + 256u + (uint32_t)(q * 16), v);
+            for (int qq = 0; qq < 4; ++qq) {
+              const int q = 4 * half + qq;
+              float v[16];
+              acc_ld16(S, qq * 16, v);
 #pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i] + s_cdir[q * 16 + i], 0.f);
-          tile_put8(xh, xl, row, 2 * q, v);
-          tile_put8(xh, xl, row, 2 * q + 1, v + 8);
-        }
-        ms.publish();
-        if (tid == 0) {
-#pragma unroll
-          for (int net = 0; net < 2; ++net) {
-            mma_chunks(tm + (uint32_t)(net * 64), sb + L.xh + (uint32_t)net * 8u * 2048u, sb + L.wa2[net], 64, 8, false);
-            mma_chunks(tm + (uint32_t)(net * 64), sb + L.xl + (uint32_t)net * 8u * 2048u, sb + L.wa2[net], 64, 8, true);
+              for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i] + s_cdir[q * 16 + i], 0.f);
+              tile_put8(xh, xl, row, 2 * q, v);
+              tile_put8(xh, xl, row, 2 * q + 1, v + 8);
+            }
           }
-          ms.commit();
+          publish();
         }
-        ms.wait();
-        x_issue_next(ray, j0 >> 7);                    // the attribute hidden tile (in the X buffer) has been consumed
         float o = 0.f;
+#pragma unroll 1
+        for (int net = 0; net < 2; ++net) {
+          mma_rows<64>(S, 0, sb + L.xh + (uint32_t)net * 8u * 2048u, sb + L.xl + (uint32_t)net * 8u * 2048u, sb + L.wa2[net], 64, 8);
+          __syncthreads();
+          if (half == net) {
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          float v[16];
-          tmem_ld16(tlane + (uint32_t)(half * 64 + q * 16), v);
+            for (int q = 0; q < 4; ++q) {
+              float v[16];
+              acc_ld16(S, q * 16, v);
 #pragma unroll
-          for (int i = 0; i < 16; ++i) o = fmaf(fmaxf(v[i], 0.f), l4d_ld1(M.att_w3[half] + q * 16 + i), o);
+              for (int i = 0; i < 16; ++i) o = fmaf(fmaxf(v[i], 0.f), l4d_ld1(M.att_w3[half] + q * 16 + i), o);
+            }
+          }
+          __syncthreads();
         }
+        x_issue_next(ray, j0 >> 7);                    // the attribute hidden tile (in the X buffer) has been consumed
         if (masked) a = l4d_sigmoid(o);
       }
       pa = fmaf(w, a, pa);
@@ -440,17 +429,12 @@ __global__ void __launch_bounds__(256) k_fwd_dense_tc(const __grid_constant__ Sp
           if (A.zvals) A.zvals[p] = zj;
         }
       }
-      tc_fence_before();
-      __syncthreads();          // TMEM columns and tiles are reused by the next tile
-      tc_fence_after();
+      __syncthreads();          // the staging tile and the operand tiles are reused by the next tile
     }
     pd = half_sum(pd, s_w); pa = half_sum(pa, s_w); pw = half_sum(pw, s_w);
     if (tid == 0) { A.depth[ray] = pd; A.image[2 * ray] = pa; A.wsum[ray] = pw; }
     if (tid == 128) A.image[2 * ray + 1] = pa;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tm, 512);
 }
 
 #ifdef L4D_PHASE_CLOCKS
@@ -460,18 +444,17 @@ __device__ unsigned long long g_phase_clk[32];
 #define L4D_PH(i) do { } while (0)
 #endif
 
-// 256 threads, two threads per row that split the columns of every epilogue (tcgen05.ld lets warps w and w+4
-// address the same TMEM lane quadrant): twice the warps to hide latency (a 128-thread, one-thread-per-row
-// version measured 4 warps/SM, IPC 0.45, stalls on long_scoreboard / wait / instruction fetch).
+// 256 threads, two threads per row that split the columns of every epilogue: twice the warps to hide latency, and one
+// warpgroup per 64-row block of every 128-sample product.
 __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ SplitArgs A) {
   using namespace l4dtc;
-  extern __shared__ __align__(1024) unsigned char dsm[];
-  __shared__ __align__(8) uint64_t s_bar, s_xbar;
-  __shared__ uint32_t s_tmem;
+  extern __shared__ __align__(128) unsigned char dsm[];
+  __shared__ __align__(8) uint64_t s_xbar;
   const DevModel& M = A.M;
   const DevGrads& G = A.G;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int row = tid & 127, half = tid >> 7, wq = warp & 3;     // two threads per row: `half` owns columns [32*half, 32*half+32) of every 64-wide block
+  const int tid = threadIdx.x;
+  const int row = tid & 127, half = tid >> 7;     // two threads per row: `half` owns columns [32*half, 32*half+32) of every 64-wide block
+  const int wg = half;                            // warpgroup
   const uint32_t in_pad = M.sigma_in_pad;
   const DenseBwdSmem L = dense_bwd_smem(in_pad);
   const uint32_t sb = smem_u32(dsm);
@@ -495,8 +478,10 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
   float* s_csum = s_cdir2 + 128;
   float* s_w = s_csum + 128;
   float* s_tstart = s_w + 32;
+  float* S = reinterpret_cast<float*>(dsm + L.acc);
+  // the attribute phase's per-row dot-product exchange lives in the dO8 tile, which is dead while it is used
+  float* s_part = reinterpret_cast<float*>(o8h);
   __shared__ float s_w3max[2];
-  __shared__ float s_part[256];
 #ifdef L4D_PHASE_CLOCKS
   __shared__ unsigned long long s_clk[32];
   long long t_last = clock64();
@@ -504,8 +489,7 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
   __syncthreads();
 #endif
 
-  if (tid == 0) { mbar_init(&s_bar, 1); mbar_init(&s_xbar, 1); fence_mbar_init(); }
-  if (warp == 0) tmem_alloc(&s_tmem, 512);
+  if (tid == 0) { mbar_init(&s_xbar, 1); fence_mbar_init(); }
   if (tid < 2) {
     float m = 1.0f;
     for (int k = 0; k < 64; ++k) m = fmaxf(m, fabsf(l4d_ld1(M.att_w3[tid] + k)));
@@ -523,17 +507,12 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
     cp(L.wa2[0], M.tc_att_w2[0], 64 * 64 * 2);
     cp(L.wa2[1], M.tc_att_w2[1], 64 * 64 * 2);
   }
-  MmaSync ms{&s_bar, 0u};
-  ms.publish();
-  const uint32_t tm = s_tmem;
-  const uint32_t tlane = tm + ((uint32_t)(wq * 32) << 16);
+  publish();
   const RaySampling rs = l4d_make_sampling(M.near_lidar, M.far_lidar, A.S, A.perturb, A.seed);
-  const uint32_t S = A.S;
-  const int n_tiles = (int)((S + 127) / 128);
+  const uint32_t n_steps = A.S;
+  const int n_tiles = (int)((n_steps + 127) / 128);
   const float kk = M.active_sensor ? 2.0f : 1.0f;
   const int n_xchunks = (int)in_pad / 8;
-  const int row64 = wq * 16 + lane;            // row held by this thread in an M=64 accumulator (lanes < 16)
-  const bool has64 = lane < 16;
 
   // The X tile (fp16 hi|lo operand tile written by k_fwd_gather) arrives by bulk copy.  It is needed twice per tile
   // (forward recompute, first-layer weight gradient) and the attribute phase reuses its buffer in between, so:
@@ -592,15 +571,15 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
     float suffix = 0.f;
     for (int t = n_tiles - 1; t >= 0; --t) {
       const uint32_t j = (uint32_t)t * 128 + row;
-      const bool active = j < S;
-      const size_t p = (size_t)ray * S + (active ? j : 0);
+      const bool active = j < n_steps;
+      const size_t p = (size_t)ray * n_steps + (active ? j : 0);
       bool masked = false;
       float dsigma = 0.f, da[2] = {0.f, 0.f};
       {
         float v = 1.f, alpha = 0.f, gw = 0.f, delta = 0.f;
         if (active) {
           const float zj = l4d_z(rs, rg, j);
-          delta = (j + 1 < S) ? (l4d_z(rs, rg, j + 1) - zj) : rs.sample_dist;
+          delta = (j + 1 < n_steps) ? (l4d_z(rs, rg, j + 1) - zj) : rs.sample_dist;
           alpha = l4d_alpha(M, delta, A.sv.sigma[p]);
           v = (1.0f - alpha) + 1e-15f;
           gw = gd * zj + gi0 * A.sv.attr[p] + gi1 * A.sv.attr[A.sv.P + p] + gws;
@@ -621,20 +600,16 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
       L4D_PH(1);
       // ---------------- P1: sigma MLP forward ----------------
       x_wait();
-      ms.publish();
+      publish();
       L4D_PH(2);
-      if (tid == 0) {
-        mma_chunks(tm + 0, aXh, sb + L.w1, 64, n_xchunks, false);
-        mma_chunks(tm + 0, aXl, sb + L.w1, 64, n_xchunks, true);
-        ms.commit();
-      }
-      ms.wait();
+      mma_rows<64>(S, 0, aXh, aXl, sb + L.w1, 64, n_xchunks);
+      __syncthreads();
       uint32_t msk = 0u;                       // relu pattern of this half's 32 hidden units
 #pragma unroll
       for (int qq = 0; qq < 2; ++qq) {
         const int q = 2 * half + qq;
         float v[16];
-        tmem_ld16(tlane + (uint32_t)(q * 16), v);
+        acc_ld16(S, q * 16, v);
 #pragma unroll
         for (int i = 0; i < 16; ++i) {
           const bool on = v[i] > 0.f;
@@ -644,15 +619,11 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
         tile_put8(hh, hl, row, 2 * q, v);
         tile_put8(hh, hl, row, 2 * q + 1, v + 8);
       }
-      ms.publish();
-      if (tid == 0) {
-        mma_chunks(tm + 128, aHh, sb + L.w2, 16, 8, false);
-        mma_chunks(tm + 128, aHl, sb + L.w2, 16, 8, true);
-        ms.commit();
-      }
-      ms.wait();
+      publish();
+      mma_rows<16>(S, 0, aHh, aHl, sb + L.w2, 16, 8);
+      __syncthreads();
       float out[16], dgeo[16];
-      tmem_ld16(tlane + 128u, out);
+      acc_ld16(S, 0, out);
 #pragma unroll
       for (int i = 0; i < 16; ++i) dgeo[i] = 0.f;
 
@@ -674,19 +645,15 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
         for (int net = 0; net < 2; ++net) {
           if (block_amax256(da[net], s_w) == 0.f) continue;       // no gradient reaches this head in this tile
           x_dirty = true;
-          ms.publish();
-          if (tid == 0) {
-            mma_chunks(tm + 0, aG16h, sb + L.wa1[net], 64, 2, false);
-            mma_chunks(tm + 0, aG16l, sb + L.wa1[net], 64, 2, true);
-            ms.commit();
-          }
-          ms.wait();
+          publish();
+          mma_rows<64>(S, 0, aG16h, aG16l, sb + L.wa1[net], 64, 2);
+          __syncthreads();
           uint32_t m1 = 0u;
 #pragma unroll
           for (int qq = 0; qq < 2; ++qq) {
             const int q = 2 * half + qq;
             float v[16];
-            tmem_ld16(tlane + (uint32_t)(q * 16), v);
+            acc_ld16(S, q * 16, v);
 #pragma unroll
             for (int i = 0; i < 16; ++i) {
               const float y = v[i] + s_cdir2[net * 64 + q * 16 + i];
@@ -697,13 +664,9 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
             tile_put8(t1h, t1l, row, 2 * q, v);
             tile_put8(t1h, t1l, row, 2 * q + 1, v + 8);
           }
-          ms.publish();
-          if (tid == 0) {
-            mma_chunks(tm + 64, aT1h, sb + L.wa2[net], 64, 8, false);
-            mma_chunks(tm + 64, aT1l, sb + L.wa2[net], 64, 8, true);
-            ms.commit();
-          }
-          ms.wait();
+          publish();
+          mma_rows<64>(S, 0, aT1h, aT1l, sb + L.wa2[net], 64, 8);
+          __syncthreads();
           float cs = 1.0f;
           {   // output layer (fp32), sigmoid backward, delta of the second hidden layer
             float o = 0.f;
@@ -712,7 +675,7 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
             for (int qq = 0; qq < 2; ++qq) {
               const int q = 2 * half + qq;
               float v[16];
-              tmem_ld16(tlane + 64u + (uint32_t)(q * 16), v);
+              acc_ld16(S, q * 16, v);
 #pragma unroll
               for (int i = 0; i < 16; ++i) {
                 const bool on = v[i] > 0.f;
@@ -745,30 +708,27 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
               tile_put8(t3h, t3l, row, q, v);
             }
           }
-          ms.publish();
-          if (tid == 0) {
-            // dw3^T[64 x 8] = H2^T * dO
-            mma_tt(tm + 176, aT2h, 64, aO8h, 8, false);
-            mma_tt(tm + 176, aT2l, 64, aO8h, 8, true);
-            mma_tt(tm + 176, aT2h, 64, aO8l, 8, true);
-            // dW2^T[64 x 64] = H1^T * dH2
-            mma_tt(tm + 192, aT1h, 64, aT3h, 64, false);
-            mma_tt(tm + 192, aT1l, 64, aT3h, 64, true);
-            mma_tt(tm + 192, aT1h, 64, aT3l, 64, true);
-            // dH1[128 x 64] = dH2 * W2
-            mma_prop(tm + 0, aT3h, 8, sb + L.wa2[net], 64, 64, false);
-            mma_prop(tm + 0, aT3l, 8, sb + L.wa2[net], 64, 64, true);
-            ms.commit();
-          }
-          ms.wait();
+          publish();
           const float inv = 1.0f / cs;
+          // dw3^T[64 x 8] = H2^T * dO (column 0 carries dO; warpgroup 0)
+          if (wg == 0)
+            mma_tt<8>(aT2h, aT2l, aO8h, aO8l, [&](int r, int c, float x, float) {
+              if (c == 0) atomicAdd(G.att_w3[net] + r, x * inv);
+            });
+          // dW2^T[64 x 64] = H1^T * dH2 (warpgroup w: columns [32w, 32w + 32))
+          mma_tt<32>(aT1h, aT1l, aT3h + (uint32_t)wg * 4u * 2048u, aT3l + (uint32_t)wg * 4u * 2048u, [&](int r, int c, float x, float y) {
+            red2(G.att_w2t[net] + (size_t)r * 64 + 32 * wg + c, x * inv, y * inv);
+          });
+          // dH1[128 x 64] = dH2 * W2
+          mma_prop<64>(S, 0, aT3h, aT3l, 8, sb + L.wa2[net], 64);
+          __syncthreads();
           float cs2;
           {   // re-scale the propagated delta with its own amax, then dH1 * relu1 -> T2 (H2 is dead)
             float am = 0.f;
             float vv[2][16];
 #pragma unroll
             for (int qq = 0; qq < 2; ++qq) {
-              tmem_ld16(tlane + (uint32_t)((2 * half + qq) * 16), vv[qq]);
+              acc_ld16(S, (2 * half + qq) * 16, vv[qq]);
 #pragma unroll
               for (int i = 0; i < 16; ++i) {
                 vv[qq][i] = ((m1 >> (qq * 16 + i)) & 1u) ? vv[qq][i] : 0.f;
@@ -789,52 +749,25 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
           }
           const float inv2 = 1.0f / cs2;
           L4D_PH(4);
-          {   // flush dw3 and dW2^T (rows live in lanes < 16 of every warp; columns split between the halves)
-            float v[16];
-            tmem_ld16(tlane + 176u, v);        // 8 valid columns; column 0 = dw3[row]
-            if (has64 && half == 0) atomicAdd(G.att_w3[net] + row64, v[0] * inv);
-#pragma unroll
-            for (int qq = 0; qq < 2; ++qq) {
-              const int q = 2 * half + qq;
-              tmem_ld16(tlane + 192u + (uint32_t)(q * 16), v);
-              if (has64) {
-#pragma unroll
-                for (int i = 0; i < 16; i += 4)
-                  l4d_red4(G.att_w2t[net] + (size_t)row64 * 64 + q * 16 + i, v[i] * inv, v[i + 1] * inv, v[i + 2] * inv, v[i + 3] * inv);
-              }
-            }
-          }
           L4D_PH(5);
-          ms.publish();
-          if (tid == 0) {
-            // dW1g[64 x 16] = dH1^T * [geo,1]
-            mma_tt(tm + 160, aT2h, 64, aG16h, 16, false);
-            mma_tt(tm + 160, aT2l, 64, aG16h, 16, true);
-            mma_tt(tm + 160, aT2h, 64, aG16l, 16, true);
-            // dG[128 x 16] = dH1 * W1g
-            mma_prop(tm + 128, aT2h, 8, sb + L.wa1[net], 64, 16, false);
-            mma_prop(tm + 128, aT2l, 8, sb + L.wa1[net], 64, 16, true);
-            ms.commit();
-          }
-          ms.wait();
+          publish();
+          // dW1g[64 x 16] = dH1^T * [geo,1] (warpgroup w: columns [8w, 8w + 8); column 15 is the ones column)
+          mma_tt<8>(aT2h, aT2l, aG16h + (uint32_t)wg * 2048u, aG16l + (uint32_t)wg * 2048u, [&](int r, int c, float x, float y) {
+            const int ii = 8 * wg + c;
+            atomicAdd(G.att_w1t[net] + (size_t)(L4D_ENC + ii) * 64 + r, x * inv2);
+            if (ii + 1 < 15) atomicAdd(G.att_w1t[net] + (size_t)(L4D_ENC + ii + 1) * 64 + r, y * inv2);
+            else s_csum[net * 64 + r] += y * inv2;
+          });
+          // dG[128 x 16] = dH1 * W1g
+          mma_prop<16>(S, 0, aT2h, aT2l, 8, sb + L.wa1[net], 64);
+          __syncthreads();
           {
             float v[16];
-            tmem_ld16(tlane + 128u, v);
+            acc_ld16(S, 0, v);
 #pragma unroll
             for (int i = 0; i < 15; ++i) dgeo[i] = fmaf(v[i], inv2, dgeo[i]);
-            tmem_ld16(tlane + 160u, v);
-            if (has64) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const int ii = 8 * half + i;
-                if (ii < 15) atomicAdd(G.att_w1t[net] + (size_t)(L4D_ENC + ii) * 64 + row64, (half ? v[8 + i] : v[i]) * inv2);
-              }
-              if (half == 1) s_csum[net * 64 + row64] += v[15] * inv2;
-            }
           }
-          tc_fence_before();
           __syncthreads();
-          tc_fence_after();
           L4D_PH(6);
         }
       }
@@ -851,9 +784,7 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
       float* dq = A.sv.dfeat + l4d_dfeat_off(A.sv, ray, j);     // this row in the dfeat tile (float4 per 4 features)
       if (amax == 0.f) {           // nothing flows back through this tile
         if (active) for (int kq = half; kq < (int)A.sv.d_quads; kq += 2) *reinterpret_cast<float4*>(dq + (size_t)kq * 512) = make_float4(0.f, 0.f, 0.f, 0.f);
-        tc_fence_before();
         __syncthreads();
-        tc_fence_after();
         x_issue_next(ray, t);
         continue;
       }
@@ -868,32 +799,21 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
         for (int i = 0; i < 8; ++i) d8[i] = half ? d16[8 + i] : d16[i];
         tile_put8(o16h, o16l, row, half, d8);
       }
-      ms.publish();
-      if (tid == 0) {
-        // dHs[128 x 64] = dO * W2   (W2 stored [k/8][16 rows][8])
-        mma_prop(tm + 64, aO16h, 2, sb + L.w2, 16, 64, false);
-        mma_prop(tm + 64, aO16l, 2, sb + L.w2, 16, 64, true);
-        // dW2s^T[64 x 16] = Hs^T * dO
-        mma_tt(tm + 144, aHh, 64, aO16h, 16, false);
-        mma_tt(tm + 144, aHl, 64, aO16h, 16, true);
-        mma_tt(tm + 144, aHh, 64, aO16l, 16, true);
-        ms.commit();
-      }
-      ms.wait();
-      {
-        float v[16];
-        tmem_ld16(tlane + 144u, v);
-        if (has64) {
-#pragma unroll
-          for (int o = 0; o < 8; ++o) atomicAdd(G.sig_w2 + (size_t)(8 * half + o) * 64 + row64, (half ? v[8 + o] : v[o]) * inv);
-        }
-      }
+      publish();
+      // dHs[128 x 64] = dO * W2   (W2 stored [k/8][16 rows][8])
+      mma_prop<64>(S, 0, aO16h, aO16l, 2, sb + L.w2, 16);
+      // dW2s^T[64 x 16] = Hs^T * dO (warpgroup w: columns [8w, 8w + 8))
+      mma_tt<8>(aHh, aHl, aO16h + (uint32_t)wg * 2048u, aO16l + (uint32_t)wg * 2048u, [&](int r, int c, float x, float y) {
+        atomicAdd(G.sig_w2 + (size_t)(8 * wg + c) * 64 + r, x * inv);
+        atomicAdd(G.sig_w2 + (size_t)(8 * wg + c + 1) * 64 + r, y * inv);
+      });
+      __syncthreads();
       {   // re-scale the propagated delta with its own amax, then dHs * relu -> RH (hidden is dead)
         float am2 = 0.f;
         float vv[2][16];
 #pragma unroll
         for (int qq = 0; qq < 2; ++qq) {
-          tmem_ld16(tlane + 64u + (uint32_t)((2 * half + qq) * 16), vv[qq]);
+          acc_ld16(S, (2 * half + qq) * 16, vv[qq]);
 #pragma unroll
           for (int i = 0; i < 16; ++i) {
             vv[qq][i] = ((msk >> (qq * 16 + i)) & 1u) ? vv[qq][i] : 0.f;
@@ -915,65 +835,33 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
       L4D_PH(7);
       // ---------------- P4: input gradients and first-layer weight gradient ----------------
       x_wait();
-      ms.publish();
+      publish();
       L4D_PH(8);
-      if (tid == 0) {
-        // dX[128 x in_pad] = dHs * W1   (W1 stored [k/8][64 rows][8])
-        mma_prop(tm + 256, aHh, 8, sb + L.w1, 64, in_pad, false);
-        mma_prop(tm + 256, aHl, 8, sb + L.w1, 64, in_pad, true);
-        // dW1^T[in x 64] = X^T * dHs : rows 0..127, then rows 128..191
-        mma_tt(tm + 192, aXh, 128, aHh, 64, false);
-        mma_tt(tm + 192, aXl, 128, aHh, 64, true);
-        mma_tt(tm + 192, aXh, 128, aHl, 64, true);
-        if (in_pad > 128) {
-          mma_tt(tm + 448, aXh + 16u * 2048u, 64, aHh, 64, false);
-          mma_tt(tm + 448, aXl + 16u * 2048u, 64, aHh, 64, true);
-          mma_tt(tm + 448, aXh + 16u * 2048u, 64, aHl, 64, true);
-        }
-        ms.commit();
+      {
+        // dW1^T[in x 64] = X^T * dHs: feature rows [0,64) on warpgroup 0, [64,128) on warpgroup 1, [128,192) split by columns
+        auto flush = [&](int r, int c, float x, float y) {
+          if (r < (int)in_pad) red2(G.sig_w1t + (size_t)r * 64 + c, x * inv, y * inv);
+        };
+        mma_tt<64>(aXh + (uint32_t)wg * 8u * 2048u, aXl + (uint32_t)wg * 8u * 2048u, aHh, aHl,
+                   [&](int r, int c, float x, float y) { flush(64 * wg + r, c, x, y); });
+        if (in_pad > 128)
+          mma_tt<32>(aXh + 16u * 2048u, aXl + 16u * 2048u, aHh + (uint32_t)wg * 4u * 2048u, aHl + (uint32_t)wg * 4u * 2048u,
+                     [&](int r, int c, float x, float y) { flush(128 + r, 32 * wg + c, x, y); });
       }
-      ms.wait();
-      x_issue_next(ray, t);              // X is free: fetch the next tile behind this epilogue
-      L4D_PH(9);
-      for (int q = half; q < (int)in_pad / 16; q += 2) {
-        float v[16];
-        tmem_ld16(tlane + 256u + (uint32_t)(q * 16), v);
-        if (active) {
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            const int kq = q * 4 + g;
-            if (kq < (int)A.sv.d_quads)
-              *reinterpret_cast<float4*>(dq + (size_t)kq * 512) = make_float4(v[4 * g] * inv, v[4 * g + 1] * inv, v[4 * g + 2] * inv, v[4 * g + 3] * inv);
-          }
-        }
-      }
-#pragma unroll
-      for (int qq = 0; qq < 2; ++qq) {
-        const int q = 2 * half + qq;
-        float v[16];
-        tmem_ld16(tlane + 192u + (uint32_t)(q * 16), v);
-        if (row < (int)in_pad) {
-#pragma unroll
-          for (int i = 0; i < 16; i += 4)
-            l4d_red4(G.sig_w1t + (size_t)row * 64 + q * 16 + i, v[i] * inv, v[i + 1] * inv, v[i + 2] * inv, v[i + 3] * inv);
-        }
-      }
-      if (in_pad > 128) {
-#pragma unroll
-        for (int qq = 0; qq < 2; ++qq) {
-          const int q = 2 * half + qq;
-          float v[16];
-          tmem_ld16(tlane + 448u + (uint32_t)(q * 16), v);
-          if (has64 && 128 + row64 < (int)in_pad) {
-#pragma unroll
-            for (int i = 0; i < 16; i += 4)
-              l4d_red4(G.sig_w1t + (size_t)(128 + row64) * 64 + q * 16 + i, v[i] * inv, v[i + 1] * inv, v[i + 2] * inv, v[i + 3] * inv);
-          }
-        }
-      }
-      tc_fence_before();
       __syncthreads();
-      tc_fence_after();
+      x_issue_next(ray, t);              // X is free: fetch the next tile behind the input gradients
+      L4D_PH(9);
+      // dX[128 x in_pad] = dHs * W1 (W1 stored [k/8][64 rows][8]) -> dfeat, 16 columns at a time straight from the registers
+      for (int n0 = 0; n0 < (int)A.sv.d_quads * 4; n0 += 16) {
+        mma_prop_frag<16>(aHh, aHl, 8, sb + L.w1 + (uint32_t)(n0 / 8) * 64u * 16u, 64, [&](int r, int c, float x, float y) {
+          const uint32_t jr = (uint32_t)t * 128 + (uint32_t)r;
+          const int col = n0 + c;
+          if (jr < n_steps && col < (int)A.sv.d_quads * 4)
+            *reinterpret_cast<float2*>(A.sv.dfeat + l4d_dfeat_off(A.sv, ray, jr) + (size_t)(col >> 2) * 512 + (col & 3)) =
+                make_float2(x * inv, y * inv);
+        });
+      }
+      __syncthreads();
       L4D_PH(11);
     }
     // direction / ones rows of the first attribute layer: dW1t[k][j] += enc[k] * sum_samples dh1[j]
@@ -986,13 +874,11 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
       else atomicAdd(G.att_w1t[net] + (size_t)(M.attr_in_dim + (r - L4D_ENC)) * 64 + jx, cs);
     }
   }
-  tc_fence_before();
-  __syncthreads();
 #ifdef L4D_PHASE_CLOCKS
+  __syncthreads();
   L4D_PH(12);
   if (tid < 32) atomicAdd(&g_phase_clk[tid], s_clk[tid]);
 #endif
-  if (warp == 0) tmem_dealloc(tm, 512);
 }
 
 // =============================================================================================
@@ -1002,6 +888,7 @@ struct FlowTcSmem {
   uint32_t w0, w1, w2;       // weights
   uint32_t fin;              // 16-wide tile hi|lo (2 x 4 KB)
   uint32_t t1, t2;           // 64-wide tiles hi|lo (32 KB each); the forward uses t1 only
+  uint32_t acc;              // fp32 staging tile
   uint32_t do16;             // 16-wide delta tile hi|lo
   uint32_t total_fwd, total;
 };
@@ -1012,6 +899,7 @@ __host__ __device__ inline FlowTcSmem flow_tc_smem() {
   L.w0 = take(16 * 64 * 2); L.w1 = take(64 * 64 * 2); L.w2 = take(64 * 16 * 2);
   L.fin = take(2 * 4096);
   L.t1 = take(32 * 1024);
+  L.acc = take(l4dtc::acc_tile_bytes());
   L.total_fwd = o;
   L.t2 = take(32 * 1024);
   L.do16 = take(2 * 4096);
@@ -1031,11 +919,10 @@ __device__ __forceinline__ void flow_copy_weights(unsigned char* dsm, const Flow
 }
 
 // flow MLP forward for the 128 samples of the CTA.  fin[16] per thread in, flow[8] out (6 used).
-// TMEM: [tm, tm+64) layer 1, [tm+64, tm+128) layer 2, [tm, tm+16) output.  Optionally returns the relu patterns
-// and leaves relu(layer-2) in tile t1 and (when H1_OUT) relu(layer-1) in tile h1_out.
+// Optionally returns the relu patterns and leaves relu(layer-2) in tile t1 and (when H1_OUT) relu(layer-1) in tile h1_out.
 template <bool H1_OUT>
-__device__ __forceinline__ void flow_forward_tc(unsigned char* dsm, uint32_t sb, const FlowTcSmem& L, MmaSync& ms, uint32_t tm,
-                                                uint32_t tlane, const float (&fin)[16], float (&flow)[8], uint32_t& m1a,
+__device__ __forceinline__ void flow_forward_tc(unsigned char* dsm, uint32_t sb, const FlowTcSmem& L, float* S,
+                                                const float (&fin)[16], float (&flow)[8], uint32_t& m1a,
                                                 uint32_t& m1b, uint32_t& m2a, uint32_t& m2b, unsigned char* h1_hi,
                                                 unsigned char* h1_lo, uint32_t a_h1_hi, uint32_t a_h1_lo) {
   const int tid = threadIdx.x;
@@ -1044,18 +931,14 @@ __device__ __forceinline__ void flow_forward_tc(unsigned char* dsm, uint32_t sb,
   const uint32_t a_y1h = H1_OUT ? a_h1_hi : sb + L.t1, a_y1l = H1_OUT ? a_h1_lo : sb + L.t1 + 16384u;
   tile_put8(fh, fl, tid, 0, fin);
   tile_put8(fh, fl, tid, 1, fin + 8);
-  ms.publish();
-  if (tid == 0) {
-    mma_chunks(tm + 0, sb + L.fin, sb + L.w0, 64, 2, false);
-    mma_chunks(tm + 0, sb + L.fin + 4096u, sb + L.w0, 64, 2, true);
-    ms.commit();
-  }
-  ms.wait();
+  publish();
+  mma_rows<64>(S, 0, sb + L.fin, sb + L.fin + 4096u, sb + L.w0, 64, 2);
+  __syncthreads();
   m1a = m1b = m2a = m2b = 0u;
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
     float v[16];
-    tmem_ld16(tlane + (uint32_t)(q * 16), v);
+    acc_ld16(S, q * 16, v);
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
       const int k = q * 16 + i;
@@ -1066,17 +949,13 @@ __device__ __forceinline__ void flow_forward_tc(unsigned char* dsm, uint32_t sb,
     tile_put8(y1h, y1l, tid, 2 * q, v);
     tile_put8(y1h, y1l, tid, 2 * q + 1, v + 8);
   }
-  ms.publish();
-  if (tid == 0) {
-    mma_chunks(tm + 64, a_y1h, sb + L.w1, 64, 8, false);
-    mma_chunks(tm + 64, a_y1l, sb + L.w1, 64, 8, true);
-    ms.commit();
-  }
-  ms.wait();
+  publish();
+  mma_rows<64>(S, 0, a_y1h, a_y1l, sb + L.w1, 64, 8);
+  __syncthreads();
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
     float v[16];
-    tmem_ld16(tlane + 64u + (uint32_t)(q * 16), v);
+    acc_ld16(S, q * 16, v);
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
       const int k = q * 16 + i;
@@ -1087,15 +966,11 @@ __device__ __forceinline__ void flow_forward_tc(unsigned char* dsm, uint32_t sb,
     tile_put8(t1h, t1l, tid, 2 * q, v);
     tile_put8(t1h, t1l, tid, 2 * q + 1, v + 8);
   }
-  ms.publish();
-  if (tid == 0) {
-    mma_chunks(tm + 0, sb + L.t1, sb + L.w2, 16, 8, false);
-    mma_chunks(tm + 0, sb + L.t1 + 16384u, sb + L.w2, 16, 8, true);
-    ms.commit();
-  }
-  ms.wait();
+  publish();
+  mma_rows<16>(S, 0, sb + L.t1, sb + L.t1 + 16384u, sb + L.w2, 16, 8);
+  __syncthreads();
   float o[16];
-  tmem_ld16(tlane, o);
+  acc_ld16(S, 0, o);
 #pragma unroll
   for (int k = 0; k < 8; ++k) flow[k] = o[k];
 }
@@ -1107,22 +982,16 @@ __device__ __forceinline__ void flow_forward_tc(unsigned char* dsm, uint32_t sb,
 // round trips need block-wide barriers, and barriers around the long, irregular feature gathers stall warps
 // that would otherwise run free (measured: fusing them doubled the forward at L=16).
 // -------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 4) k_fwd_flow_tc(const __grid_constant__ SplitArgs A) {
+__global__ void __launch_bounds__(128, 2) k_fwd_flow_tc(const __grid_constant__ SplitArgs A) {
   using namespace l4dtc;
-  extern __shared__ __align__(1024) unsigned char dsm[];
-  __shared__ __align__(8) uint64_t s_bar;
-  __shared__ uint32_t s_tmem;
+  extern __shared__ __align__(128) unsigned char dsm[];
   const DevModel& M = A.M;
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const FlowTcSmem L = flow_tc_smem();
   const uint32_t sb = smem_u32(dsm);
-  if (tid == 0) { mbar_init(&s_bar, 1); fence_mbar_init(); }
-  if (warp == 0) tmem_alloc(&s_tmem, 128);
+  float* S = reinterpret_cast<float*>(dsm + L.acc);
   flow_copy_weights(dsm, L, M);
-  MmaSync ms{&s_bar, 0u};
-  ms.publish();
-  const uint32_t tm = s_tmem;
-  const uint32_t tlane = tm + ((uint32_t)(warp * 32) << 16);
+  publish();
   const size_t P = A.sv.P;
   const RaySampling rs = l4d_make_sampling(M.near_lidar, M.far_lidar, A.S, A.perturb, A.seed);
   for (size_t base = (size_t)blockIdx.x * 128; base < P; base += (size_t)gridDim.x * 128) {
@@ -1149,35 +1018,26 @@ __global__ void __launch_bounds__(128, 4) k_fwd_flow_tc(const __grid_constant__ 
     }
     float flow[8];
     uint32_t a, b, c, d;
-    flow_forward_tc<false>(dsm, sb, L, ms, tm, tlane, fin, flow, a, b, c, d, nullptr, nullptr, 0u, 0u);
+    flow_forward_tc<false>(dsm, sb, L, S, fin, flow, a, b, c, d, nullptr, nullptr, 0u, 0u);
     if (active) {
 #pragma unroll
       for (int k = 0; k < 6; ++k) A.sv.flow[(size_t)k * P + p] = flow[k];
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tm, 128);
 }
 
 // -------------------------------------------------------------------------------------------
 // backward 3/4 on tensor cores: flow MLP backprop + weight gradients; dL/d(flow-MLP input) -> flow_in planes
-// TMEM (256 cols): [0,64) [64,128) work, [128,144) dW2^T, [144,160) dW0, [192,256) dW1^T
-// Two 64-wide tiles are enough (each delta tile overwrites the activation tile that has just been consumed), which
-// keeps the CTA at 92 KB of shared memory and 256 TMEM columns: two CTAs per SM overlap each other's MMA round trips.
+// Two 64-wide tiles are enough (each delta tile overwrites the activation tile that has just been consumed).
 // -------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128) k_bwd_flow_tc(const __grid_constant__ SplitArgs A) {
   using namespace l4dtc;
-  extern __shared__ __align__(1024) unsigned char dsm[];
-  __shared__ __align__(8) uint64_t s_bar;
-  __shared__ uint32_t s_tmem;
+  extern __shared__ __align__(128) unsigned char dsm[];
   __shared__ float s_w[32];
   const DevModel& M = A.M;
   const DevGrads& G = A.G;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x;
   const FlowTcSmem L = flow_tc_smem();
   const uint32_t sb = smem_u32(dsm);
   unsigned char *t1h = dsm + L.t1, *t1l = t1h + 16384, *t2h = dsm + L.t2, *t2l = t2h + 16384;
@@ -1185,15 +1045,9 @@ __global__ void __launch_bounds__(128) k_bwd_flow_tc(const __grid_constant__ Spl
   const uint32_t aFinH = sb + L.fin, aFinL = aFinH + 4096u;
   const uint32_t aT1h = sb + L.t1, aT1l = aT1h + 16384u, aT2h = sb + L.t2, aT2l = aT2h + 16384u;
   const uint32_t aO16h = sb + L.do16, aO16l = aO16h + 4096u;
-  if (tid == 0) { mbar_init(&s_bar, 1); fence_mbar_init(); }
-  if (warp == 0) tmem_alloc(&s_tmem, 256);
+  float* S = reinterpret_cast<float*>(dsm + L.acc);
   flow_copy_weights(dsm, L, M);
-  MmaSync ms{&s_bar, 0u};
-  ms.publish();
-  const uint32_t tm = s_tmem;
-  const uint32_t tlane = tm + ((uint32_t)(warp * 32) << 16);
-  const int row64 = warp * 16 + lane;
-  const bool has64 = lane < 16;
+  publish();
   const size_t P = A.sv.P;
   const RaySampling rs = l4d_make_sampling(M.near_lidar, M.far_lidar, A.S, A.perturb, A.seed);
   for (size_t base = (size_t)blockIdx.x * 128; base < P; base += (size_t)gridDim.x * 128) {
@@ -1219,39 +1073,28 @@ __global__ void __launch_bounds__(128) k_bwd_flow_tc(const __grid_constant__ Spl
     // forward recompute: relu(layer 1) -> T2, relu(layer 2) -> T1, relu patterns
     float flow[8];
     uint32_t m1a, m1b, m2a, m2b;
-    flow_forward_tc<true>(dsm, sb, L, ms, tm, tlane, fin, flow, m1a, m1b, m2a, m2b, t2h, t2l, aT2h, aT2l);
+    flow_forward_tc<true>(dsm, sb, L, S, fin, flow, m1a, m1b, m2a, m2b, t2h, t2l, aT2h, aT2l);
     const float sc = pow2_factor(am);
     float inv = 1.0f / sc;
 #pragma unroll
     for (int k = 0; k < 16; ++k) g[k] *= sc;
     tile_put8(o16h, o16l, tid, 0, g);
     tile_put8(o16h, o16l, tid, 1, g + 8);
-    ms.publish();
-    if (tid == 0) {
-      // dH2[128 x 64] = dO * W2 (W2 stored [k/8][16 rows][8]) ; dW2^T[64 x 16] = H2^T * dO
-      mma_prop(tm + 0, aO16h, 2, sb + L.w2, 16, 64, false);
-      mma_prop(tm + 0, aO16l, 2, sb + L.w2, 16, 64, true);
-      mma_tt(tm + 128, aT1h, 64, aO16h, 16, false);
-      mma_tt(tm + 128, aT1l, 64, aO16h, 16, true);
-      mma_tt(tm + 128, aT1h, 64, aO16l, 16, true);
-      ms.commit();
-    }
-    ms.wait();
-    {
-      float v[16];
-      tmem_ld16(tlane + 128u, v);
-      if (has64) {
-#pragma unroll
-        for (int o = 0; o < 6; ++o) atomicAdd(G.flo_w2 + (size_t)o * 64 + row64, v[o] * inv);
-      }
-    }
+    publish();
+    // dH2[128 x 64] = dO * W2 (W2 stored [k/8][16 rows][8]) ; dW2^T[64 x 16] = H2^T * dO
+    mma_prop<64>(S, 0, aO16h, aO16l, 2, sb + L.w2, 16);
+    mma_tt<16>(aT1h, aT1l, aO16h, aO16l, [&](int r, int c, float x, float y) {
+      if (c < 6) atomicAdd(G.flo_w2 + (size_t)c * 64 + r, x * inv);
+      if (c + 1 < 6) atomicAdd(G.flo_w2 + (size_t)(c + 1) * 64 + r, y * inv);
+    });
+    __syncthreads();
     float cs2;
     {   // dH2 * relu2, re-scaled -> T1 (H2 is dead: dW2^T has been computed)
       float a2 = 0.f;
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         float v[16];
-        tmem_ld16(tlane + (uint32_t)(q * 16), v);
+        acc_ld16(S, q * 16, v);
 #pragma unroll
         for (int i = 0; i < 16; ++i) if (l4d_bit(m2a, m2b, q * 16 + i)) a2 = fmaxf(a2, fabsf(v[i]));
       }
@@ -1261,7 +1104,7 @@ __global__ void __launch_bounds__(128) k_bwd_flow_tc(const __grid_constant__ Spl
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         float v[16];
-        tmem_ld16(tlane + (uint32_t)(q * 16), v);
+        acc_ld16(S, q * 16, v);
 #pragma unroll
         for (int i = 0; i < 16; ++i) v[i] = l4d_bit(m2a, m2b, q * 16 + i) ? v[i] * r : 0.f;
         tile_put8(t1h, t1l, tid, 2 * q, v);
@@ -1269,34 +1112,20 @@ __global__ void __launch_bounds__(128) k_bwd_flow_tc(const __grid_constant__ Spl
       }
     }
     inv = 1.0f / cs2;
-    ms.publish();
-    if (tid == 0) {
-      // dH1[128 x 64] = dH2 * W1 ; dW1^T[64 x 64] = H1^T * dH2
-      mma_prop(tm + 64, aT1h, 8, sb + L.w1, 64, 64, false);
-      mma_prop(tm + 64, aT1l, 8, sb + L.w1, 64, 64, true);
-      mma_tt(tm + 192, aT2h, 64, aT1h, 64, false);
-      mma_tt(tm + 192, aT2l, 64, aT1h, 64, true);
-      mma_tt(tm + 192, aT2h, 64, aT1l, 64, true);
-      ms.commit();
-    }
-    ms.wait();
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      float v[16];
-      tmem_ld16(tlane + 192u + (uint32_t)(q * 16), v);
-      if (has64) {
-#pragma unroll
-        for (int i = 0; i < 16; i += 4)
-          l4d_red4(G.flo_w1t + (size_t)row64 * 64 + q * 16 + i, v[i] * inv, v[i + 1] * inv, v[i + 2] * inv, v[i + 3] * inv);
-      }
-    }
+    publish();
+    // dH1[128 x 64] = dH2 * W1 ; dW1^T[64 x 64] = H1^T * dH2
+    mma_prop<64>(S, 0, aT1h, aT1l, 8, sb + L.w1, 64);
+    mma_tt<64>(aT2h, aT2l, aT1h, aT1l, [&](int r, int c, float x, float y) {
+      red2(G.flo_w1t + (size_t)r * 64 + c, x * inv, y * inv);
+    });
+    __syncthreads();
     float cs3;
     {   // dH1 * relu1, re-scaled -> T2 (H1 is dead: dW1^T has been computed)
       float a3 = 0.f;
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         float v[16];
-        tmem_ld16(tlane + 64u + (uint32_t)(q * 16), v);
+        acc_ld16(S, q * 16, v);
 #pragma unroll
         for (int i = 0; i < 16; ++i) if (l4d_bit(m1a, m1b, q * 16 + i)) a3 = fmaxf(a3, fabsf(v[i]));
       }
@@ -1306,7 +1135,7 @@ __global__ void __launch_bounds__(128) k_bwd_flow_tc(const __grid_constant__ Spl
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         float v[16];
-        tmem_ld16(tlane + 64u + (uint32_t)(q * 16), v);
+        acc_ld16(S, q * 16, v);
 #pragma unroll
         for (int i = 0; i < 16; ++i) v[i] = l4d_bit(m1a, m1b, q * 16 + i) ? v[i] * r : 0.f;
         tile_put8(t2h, t2l, tid, 2 * q, v);
@@ -1314,38 +1143,22 @@ __global__ void __launch_bounds__(128) k_bwd_flow_tc(const __grid_constant__ Spl
       }
     }
     inv = 1.0f / cs3;
-    ms.publish();
-    if (tid == 0) {
-      // dFin[128 x 16] = dH1 * W0 ; dW0[64 x 16] = dH1^T * Fin
-      mma_prop(tm + 0, aT2h, 8, sb + L.w0, 64, 16, false);
-      mma_prop(tm + 0, aT2l, 8, sb + L.w0, 64, 16, true);
-      mma_tt(tm + 144, aT2h, 64, aFinH, 16, false);
-      mma_tt(tm + 144, aT2l, 64, aFinH, 16, true);
-      mma_tt(tm + 144, aT2h, 64, aFinL, 16, true);
-      ms.commit();
-    }
-    ms.wait();
+    publish();
+    // dFin[128 x 16] = dH1 * W0 ; dW0[64 x 16] = dH1^T * Fin
+    mma_prop<16>(S, 0, aT2h, aT2l, 8, sb + L.w0, 64);
+    mma_tt<16>(aT2h, aT2l, aFinH, aFinL, [&](int r, int c, float x, float y) {
+      atomicAdd(G.flo_w0t + (size_t)c * 64 + r, x * inv);
+      atomicAdd(G.flo_w0t + (size_t)(c + 1) * 64 + r, y * inv);
+    });
+    __syncthreads();
     float dfin[16];
-    tmem_ld16(tlane, dfin);
-    {
-      float v[16];
-      tmem_ld16(tlane + 144u, v);
-      if (has64) {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) atomicAdd(G.flo_w0t + (size_t)i * 64 + row64, v[i] * inv);
-      }
-    }
+    acc_ld16(S, 0, dfin);
     if (active) {
       // dL/d(flow-MLP input) replaces the saved input in place (same thread, same addresses); k_bwd_flowgrid
       // turns it into flow-grid reductions at full occupancy
 #pragma unroll
       for (int k = 0; k < 16; ++k) A.sv.flow_in[(size_t)k * P + p] = dfin[k] * inv;
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tm, 256);
 }

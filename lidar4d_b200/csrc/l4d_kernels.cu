@@ -1,4 +1,4 @@
-// l4d_kernels.cu - sm_100a kernels and the C-ABI of liblidar4d_b200.so
+// l4d_kernels.cu - sm_90a kernels and the C-ABI of liblidar4d_b200.so
 // (include/lidar4d_b200.h).  Thread == sample; one CTA walks one ray tile by
 // tile and carries the transmittance; persistent grid over rays.
 //
@@ -247,7 +247,7 @@ __global__ void k_round_fp16(float* __restrict__ w, int n) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) w[i] = __half2float(__float2half_rn(w[i]));
 }
-// native W[n][k0 + k] (row stride ld) -> fp16 tcgen05 K-major interleaved layout [k/8][row_off + n][8], rows_total rows
+// native W[n][k0 + k] (row stride ld) -> fp16 wgmma K-major interleaved layout [k/8][row_off + n][8], rows_total rows
 __global__ void k_pack_umma(const float* __restrict__ W, int ld, int n_rows, int k0, int K, __half* __restrict__ dst,
                             int rows_total, int row_off) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -343,7 +343,7 @@ extern "C" int l4d_stage_params_ex(const L4DConfig* cfg, const L4DMasterParams* 
     Cp(m->flow_mlp[1], L.flo_w1, 64 * 64, 64 * 64);
     T(m->flow_mlp[2], 64, L.flo_w2t, 64, 8, 64, 6);
     Cp(m->flow_mlp[2], L.flo_w2, 6 * 64, 8 * 64);
-    // tensor-core operand copies (fp16, UMMA no-swizzle K-major layout).  Rows / columns these jobs never write
+    // tensor-core operand copies (fp16, no-swizzle K-major layout).  Rows / columns these jobs never write
     // (tc_att_w1g column 15, tc_flo_w2 rows 6..15) must be zero: the caller zero-fills `staged` once at allocation.
     U(m->sigma_net, ip, 64, 0, ip, L.tc_sig_w1, 64, 0);
     U(m->sigma_net + 64 * ip, 64, 16, 0, 64, L.tc_sig_w2, 16, 0);
@@ -1052,7 +1052,7 @@ static int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -1068,8 +1068,6 @@ static int check_rays(const L4DRays* r) {
   return L4D_OK;
 }
 
-// force_per_sm > 0 overrides the occupancy query: for kernels that allocate tensor memory the runtime reports one
-// CTA per SM although registers / shared memory / the 128 TMEM columns they actually allocate allow more
 template <typename K>
 static int grid_for(K kernel, int nt, size_t smem, uint32_t work, int& grid, int force_per_sm = 0) {
   // the attribute / occupancy calls cost ~10 us of host time each: remember the answer per (kernel, smem, threads) -
@@ -1139,8 +1137,19 @@ static void fill_split(SplitArgs& A, const L4DConfig* cfg, const void* staged, c
 
 #define L4D_FLAG_FUSED 1u   /* L4DRays.reserved bit 0: single-kernel path */
 
-// the tensor-core dense kernels hold a 128 x sigma_in_pad fp16 hi|lo tile in shared memory: up to 192 inputs (L <= 18)
-static bool use_tc_dense(const L4DConfig* cfg) { return cfg->mlp_fp16 && cfg->sigma_in_pad <= 192; }
+// Dynamic shared memory of the tensor-core kernels: the carve-up plus the 128-byte alignment of its base
+static size_t tc_dyn_smem(uint32_t bytes) { return (size_t)bytes + 128; }
+// the tensor-core dense kernels hold a 128 x sigma_in_pad fp16 hi|lo tile and an fp32 staging tile in shared memory;
+// on sm_90 (227 KB per CTA) the backward's carve-up fits up to 176 inputs (L <= 16)
+static bool use_tc_dense(const L4DConfig* cfg) {
+  static int optin = 0;
+  if (!optin) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  }
+  return cfg->mlp_fp16 && cfg->sigma_in_pad <= 192 && tc_dyn_smem(dense_bwd_smem(cfg->sigma_in_pad).total) + 128 <= (size_t)optin;
+}
 
 extern "C" int l4d_render_forward(const L4DConfig* cfg, const void* staged, const L4DFrame* frame, const L4DRays* rays,
                                   float* depth, float* image, float* wsum, float* weights, float* zvals, void* saved,
@@ -1215,9 +1224,9 @@ extern "C" int l4d_render_forward(const L4DConfig* cfg, const void* staged, cons
   }
   if (cfg->mlp_fp16) {
     {
-      const size_t smem = flow_tc_smem().total_fwd + 1024;
+      const size_t smem = tc_dyn_smem(flow_tc_smem().total_fwd);
       int grid;
-      rc = grid_for(k_fwd_flow_tc, 128, smem, (uint32_t)((P + 127) / 128), grid, 4);
+      rc = grid_for(k_fwd_flow_tc, 128, smem, (uint32_t)((P + 127) / 128), grid);
       if (rc != L4D_OK) return rc;
       ++g_launches; k_fwd_flow_tc<<<grid, 128, smem, st>>>(A);
       prof_mark(st, "k_fwd_flow_tc");
@@ -1244,7 +1253,7 @@ extern "C" int l4d_render_forward(const L4DConfig* cfg, const void* staged, cons
     prof_mark(st, "k_fwd_gather");
   }
   if (use_tc_dense(cfg)) {
-    const size_t smem = dense_fwd_smem(cfg->sigma_in_pad).total + 1024;
+    const size_t smem = tc_dyn_smem(dense_fwd_smem(cfg->sigma_in_pad).total);
     int grid;
     rc = grid_for(k_fwd_dense_tc, 256, smem, rays->n_rays, grid);
     if (rc != L4D_OK) return rc;
@@ -1302,7 +1311,7 @@ extern "C" int l4d_render_backward_ex(const L4DConfig* cfg, const void* staged, 
     const size_t P = (size_t)rays->n_rays * rays->n_steps;
     const uint32_t tiles = (uint32_t)((P + L4D_NT - 1) / L4D_NT);
     if (use_tc_dense(cfg)) {
-      const size_t smem = dense_bwd_smem(cfg->sigma_in_pad).total + 1024;
+      const size_t smem = tc_dyn_smem(dense_bwd_smem(cfg->sigma_in_pad).total);
       int grid;
       rc = grid_for(k_bwd_dense_tc, 256, smem, rays->n_rays, grid);
       if (rc != L4D_OK) return rc;
@@ -1379,9 +1388,9 @@ extern "C" int l4d_render_backward_ex(const L4DConfig* cfg, const void* staged, 
     }
     if (frame->has_fwd || frame->has_bwd) {     // with no neighbour frame nothing reaches the flow field
       if (cfg->mlp_fp16) {
-        const size_t smem = flow_tc_smem().total + 1024;
+        const size_t smem = tc_dyn_smem(flow_tc_smem().total);
         int grid;
-        rc = grid_for(k_bwd_flow_tc, 128, smem, tiles, grid, 2);     // 92 KB + 256 TMEM columns: two per SM
+        rc = grid_for(k_bwd_flow_tc, 128, smem, tiles, grid);
         if (rc != L4D_OK) return rc;
         ++g_launches; k_bwd_flow_tc<<<grid, 128, smem, st>>>(A);
         prof_mark(st, "k_bwd_flow_tc");
@@ -1526,7 +1535,7 @@ extern "C" int l4d_attribute_forward(const L4DConfig* cfg, const void* staged, c
   return L4D_OK;
 }
 
-// tcgen05 self-test: C[128][N] = A[128][K] (fp16) * B[N][K]^T (fp16), fp32 accumulate in TMEM
+// wgmma self-test: C[128][N] = A[128][K] (fp16) * B[N][K]^T (fp16), fp32 accumulate
 extern "C" int l4d_tc_selftest(const void* A, const void* B, float* Cout, uint32_t N, uint32_t K, void* stream) {
   if (!A || !B || !Cout) return l4d_fail(L4D_EINVAL, "null pointer");
   if (N < 16 || N > 256 || N % 16 || K < 16 || K % 16 || K > 512) return l4d_fail(L4D_EINVAL, "need N%16==0 in [16,256], K%16==0 in [16,512]");
@@ -1538,7 +1547,7 @@ extern "C" int l4d_tc_selftest(const void* A, const void* B, float* Cout, uint32
   return L4D_OK;
 }
 
-// tcgen05 self-test 2: operands pre-arranged in tile format; M in {64,128}; either operand may be MN-major
+// wgmma self-test 2: operands pre-arranged in tile format; M in {64,128}; either operand may be MN-major
 extern "C" int l4d_tc_selftest2(const void* A, const void* B, float* Cout, uint32_t M, uint32_t N, uint32_t K,
                                 uint32_t a_mn, uint32_t b_mn, void* stream) {
   if (!A || !B || !Cout) return l4d_fail(L4D_EINVAL, "null pointer");

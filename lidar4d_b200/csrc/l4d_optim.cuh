@@ -4,7 +4,7 @@
 //     eps 1e-15) that ALSO writes the fp16 working copies of the hash tables the render kernels gather from
 //     (static / flow: straight casts; dynamic: the two slice-pair records an entry lives in), so the 300 MB of
 //     tables are read once per step instead of three times;
-//   * k_stage_jobs / k_unstage_jobs: every small staging op (planes -> channels-last, MLP transposes, UMMA operand
+//   * k_stage_jobs / k_unstage_jobs: every small staging op (planes -> channels-last, MLP transposes, tensor-core operand
 //     packing) and every gradient fold-back in ONE launch each, driven by a job table in kernel-parameter space
 //     (they were ~55 and ~35 separate launches: ~0.4 ms of pure launch latency at the reference's 1,024-ray step).
 #pragma once

@@ -466,8 +466,8 @@ __global__ void __launch_bounds__(NT, 4) k_bwd_flowgrid(const __grid_constant__ 
 
 // -------------------------------------------------------------------------------------------
 // backward 2b: static-hash reductions, LEVEL-MAJOR.  The fp32 gradient of the static table is 8 MB per level
-// (134 MB at L=16, more than the 126 MB L2): walking all levels per sample made the reductions miss in L2
-// (ncu: 31 GB of DRAM traffic, L2 hit 59 %).  Here every CTA sweeps the samples once per level, so the whole
+// (134 MB at L=16, far more than the 50 MB L2): walking all levels per sample makes the reductions miss in L2.
+// Here every CTA sweeps the samples once per level, so the whole
 // chip works on one level at a time and its gradient slab stays L2-resident.
 // -------------------------------------------------------------------------------------------
 // L4D_STATIC_AGG_RES (0 = off): at the coarsest levels consecutive samples of a ray share their cell for 2-4 samples (res 512-1200

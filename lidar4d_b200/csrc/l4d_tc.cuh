@@ -1,12 +1,15 @@
-// l4d_tc.cuh - tcgen05 / TMEM / mbarrier building blocks for sm_100a (inline PTX).
+// l4d_tc.cuh - wgmma / mbarrier / bulk-copy building blocks for sm_90a (inline PTX).
 //
-// Tile convention used by the MLP engine: M = 128 samples (TMEM lane == sample ==
-// thread), operands fp16 K-major in shared memory in the canonical *interleaved*
-// (no-swizzle) layout: 16-byte chunks of 8 halves along K, [chunk][row] order:
+// Tile convention used by the MLP engine: M = 128 samples, operands fp16 in shared memory in the canonical
+// *interleaved* (no-swizzle) layout: 16-byte chunks of 8 halves along K, [chunk][row] order:
 //     byte(row, k) = (k/8) * (ROWS*16) + row*16 + (k%8)*2
-// => core matrix = 8 rows x 16 B contiguous, SBO (next 8 rows) = 128 B,
-//    LBO (next K chunk) = ROWS*16 B.  A thread that owns a row writes one
-//    16-byte chunk per store: conflict-free.
+// => core matrix = 8 rows x 16 B contiguous; K-major: LBO (next K chunk) = ROWS*16 B, SBO (next 8 rows) = 128 B.
+// A thread that owns a row writes one 16-byte chunk per store: conflict-free.
+//
+// MMAs are warpgroup-wide (wgmma.mma_async, m64nNk16, fp32 accumulators in registers).  A 128-row product is two
+// 64-row blocks; in a 256-thread CTA each warpgroup computes one.  Epilogues that work on whole rows (thread == row)
+// read the accumulators from an fp32 staging tile in shared memory (AccTile); weight-gradient products are flushed
+// straight from the registers.
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -43,62 +46,106 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_saddr, const void* src, ui
 // generic-proxy shared-memory writes -> visible to the async proxy (tensor core operand reads)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---- TMEM ----------------------------------------------------------------------------------
-// whole-warp calls (.sync.aligned); ncols power of two >= 32
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
 // ---- descriptors ---------------------------------------------------------------------------
-// shared-memory matrix descriptor, K-major, SWIZZLE_NONE, version 1 (Blackwell)
+// wgmma shared-memory matrix descriptor, no swizzle.  K-major: LBO = stride of the next 8-wide K chunk, SBO = stride of
+// the next 8 rows.  MN-major: LBO = stride of the next 8 K rows, SBO = stride of the next 8-wide MN chunk.
 __device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFFu);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
   return d;
 }
-// instruction descriptor: kind::f16, A/B = F16, D = F32, M x N; a_mn / b_mn = 1 selects an MN-major operand
-__host__ __device__ constexpr uint32_t idesc_f16(uint32_t M, uint32_t N, uint32_t a_mn = 0, uint32_t b_mn = 0) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | (a_mn << 15) | (b_mn << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-// TMEM lane that holds accumulator row m: M=128 -> lane m; M=64 -> 16 lanes of every 32-lane sub-partition
-__host__ __device__ constexpr uint32_t tmem_lane_of_row(uint32_t M, uint32_t m) { return M == 64 ? (m & 15u) + 32u * (m >> 4) : m; }
 
-// D[tmem] (+)= A[smem] * B[smem]^T, one K=16 step; issued by ONE thread
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier when all previously issued MMAs of this thread completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+// ---- wgmma ---------------------------------------------------------------------------------
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit_wait() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
 }
 
-// ---- TMEM -> registers: lane == thread, 16 consecutive fp32 columns ----------------------------
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// D[64 x N] (+)= A[64 x 16] * B[16 x N]; TA / TB = 1 selects an MN-major operand.  acc == 0 overwrites D.
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t acc) {
+  static_assert(N == 8 || N == 16 || N == 32 || N == 64, "wgmma_f16: N in {8, 16, 32, 64}");
+  if constexpr (N == 8) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %6, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 {%0,%1,%2,%3}, %4, %5, p, 1, 1, %7, %8;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
+  } else if constexpr (N == 16) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %11, %12;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
+  } else if constexpr (N == 32) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, %19, %20;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
+  } else {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
+  }
+}
+
+// One operand of a product: start address of each term, byte step per K=16 step, LBO / SBO of its descriptor.
+struct Opnd {
+  uint32_t addr[3];
+  uint32_t kstep, lbo, sbo;
+};
+// D[64 x N] = sum over terms t of A_t * B_t over ksteps K=16 steps; warpgroup-wide, returns with D in registers
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wg_gemm(float (&d)[N / 2], const Opnd& A, const Opnd& B, int nterms, int ksteps) {
+  wg_fence();
+  for (int t = 0; t < nterms; ++t)
+    for (int k = 0; k < ksteps; ++k)
+      wgmma_f16<N, TA, TB>(d, smem_desc(A.addr[t] + (uint32_t)k * A.kstep, A.lbo, A.sbo),
+                           smem_desc(B.addr[t] + (uint32_t)k * B.kstep, B.lbo, B.sbo), (t | k) ? 1u : 0u);
+  wg_commit_wait();
+}
+// visit the accumulator fragment of a 64 x N product: f(row, col, v[col], v[col + 1]) for the thread's element pairs
+template <int N, class F>
+__device__ __forceinline__ void frag_foreach(const float (&d)[N / 2], F&& f) {
+  const int t = threadIdx.x & 127, r = 16 * (t >> 5) + ((t & 31) >> 2), c = 2 * (t & 3);
 #pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+  for (int j = 0; j < N / 8; ++j) {
+    f(r, 8 * j + c, d[4 * j], d[4 * j + 1]);
+    f(r + 8, 8 * j + c, d[4 * j + 2], d[4 * j + 3]);
+  }
+}
+
+// ---- fp32 accumulator staging tile: 128 rows x 64 columns, float4 groups XOR-swizzled by row ----------
+__host__ __device__ constexpr uint32_t acc_tile_bytes() { return 128u * 64u * 4u; }
+__device__ __forceinline__ int acc_idx(int r, int c) { return r * 64 + ((((c >> 2) ^ r) & 15) << 2) + (c & 3); }
+// fragment of rows [m0, m0 + 64), columns [c0, c0 + N) -> staging tile
+template <int N>
+__device__ __forceinline__ void acc_store(float* S, const float (&d)[N / 2], int m0, int c0) {
+  frag_foreach<N>(d, [&](int r, int c, float a, float b) {
+    *reinterpret_cast<float2*>(S + acc_idx(m0 + r, c0 + c)) = make_float2(a, b);
+  });
+}
+// this thread's row (threadIdx.x % 128), 16 consecutive columns from c0 (c0 % 4 == 0)
+__device__ __forceinline__ void acc_ld16(const float* S, int c0, float (&v)[16]) {
+  const int r = threadIdx.x & 127;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float4 q = *reinterpret_cast<const float4*>(S + acc_idx(r, c0 + 4 * i));
+    v[4 * i] = q.x; v[4 * i + 1] = q.y; v[4 * i + 2] = q.z; v[4 * i + 3] = q.w;
+  }
 }
 
 // pack 8 floats into one 16-byte chunk of fp16 (round to nearest)
@@ -114,22 +161,16 @@ __device__ __forceinline__ uint4 pack8_half(const float* f) {
 }  // namespace l4dtc
 
 // =============================================================================================
-// self-test: C[128][N] = A[128][K] * B[N][K]^T with fp16 operands, fp32 accumulate, one CTA.
-// Exercises descriptor encoding, TMEM allocation, commit/mbarrier and the 32x32b load exactly
-// as the MLP engine uses them.
+// self-test: C[128][N] = A[128][K] * B[N][K]^T with fp16 operands, fp32 accumulate, one CTA (one warpgroup).
+// Exercises the descriptor encoding and the accumulator fragment layout exactly as the MLP engine uses them.
 // =============================================================================================
 __global__ void __launch_bounds__(128) k_tc_selftest(const __half* __restrict__ A, const __half* __restrict__ B,
                                                      float* __restrict__ C, int N, int K) {
   using namespace l4dtc;
-  extern __shared__ __align__(1024) unsigned char tc_smem[];
-  __shared__ __align__(8) uint64_t bar;
-  __shared__ uint32_t tmem_base_s;
-  const int tid = threadIdx.x, warp = tid >> 5;
+  extern __shared__ __align__(128) unsigned char tc_smem[];
+  const int tid = threadIdx.x;
   unsigned char* sA = tc_smem;                         // [K/8][128][16 B]
   unsigned char* sB = tc_smem + (size_t)(K / 8) * 128 * 16;   // [K/8][N][16 B]
-  if (tid == 0) { mbar_init(&bar, 1); fence_mbar_init(); }
-  if (warp == 0) tmem_alloc(&tmem_base_s, 256);
-  // operands -> shared memory (interleaved layout)
   for (int c = 0; c < K / 8; ++c)
     *reinterpret_cast<uint4*>(sA + ((size_t)c * 128 + tid) * 16) = *reinterpret_cast<const uint4*>(A + (size_t)tid * K + c * 8);
   for (int i = tid; i < (K / 8) * N; i += 128) {
@@ -137,30 +178,18 @@ __global__ void __launch_bounds__(128) k_tc_selftest(const __half* __restrict__ 
     *reinterpret_cast<uint4*>(sB + ((size_t)c * N + n) * 16) = *reinterpret_cast<const uint4*>(B + (size_t)n * K + c * 8);
   }
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tbase = tmem_base_s;
-  if (tid == 0) {
-    const uint32_t idesc = idesc_f16(128, (uint32_t)N);
-    for (int k = 0; k < K / 16; ++k) {
-      const uint64_t da = smem_desc(smem_u32(sA) + (uint32_t)(2 * k) * 128 * 16, 128 * 16, 128);
-      const uint64_t db = smem_desc(smem_u32(sB) + (uint32_t)(2 * k) * N * 16, (uint32_t)N * 16, 128);
-      umma_f16(tbase, da, db, idesc, k > 0 ? 1u : 0u);
+  for (int mb = 0; mb < 2; ++mb)
+    for (int n0 = 0; n0 < N; n0 += 8) {
+      const Opnd a{{smem_u32(sA) + (uint32_t)mb * 1024u, 0u, 0u}, 2u * 128u * 16u, 128u * 16u, 128u};
+      const Opnd b{{smem_u32(sB) + (uint32_t)n0 * 16u, 0u, 0u}, 2u * (uint32_t)N * 16u, (uint32_t)N * 16u, 128u};
+      float d[4];
+      wg_gemm<8, 0, 0>(d, a, b, 1, K / 16);
+      frag_foreach<8>(d, [&](int r, int c, float x, float y) {
+        C[(size_t)(64 * mb + r) * N + n0 + c] = x;
+        C[(size_t)(64 * mb + r) * N + n0 + c + 1] = y;
+      });
     }
-    umma_commit(&bar);
-  }
-  mbar_wait(&bar, 0);
-  tc_fence_after();
-  for (int n0 = 0; n0 < N; n0 += 16) {
-    float v[16];
-    tmem_ld16(tbase + ((uint32_t)(warp * 32) << 16) + (uint32_t)n0, v);
-#pragma unroll
-    for (int i = 0; i < 16; ++i) C[(size_t)tid * N + n0 + i] = v[i];
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tbase, 256);
 }
 
 // =============================================================================================
@@ -168,50 +197,38 @@ __global__ void __launch_bounds__(128) k_tc_selftest(const __half* __restrict__ 
 //   K-major operand  X[rows][K]      : byte((k/8)*rows*16 + r*16 + (k%8)*2)           LBO = rows*16, SBO = 128
 //   MN-major operand X[rows=mn][K=k] : byte((mn/8)*K*16  + k*16 + (mn%8)*2)           LBO = 128,     SBO = K*16
 // =============================================================================================
+template <int TA, int TB>
+__device__ __forceinline__ void tc_selftest2_body(const unsigned char* sA, const unsigned char* sB, float* __restrict__ C, int M,
+                                                  int N, int K) {
+  using namespace l4dtc;
+  for (int mb = 0; mb < M / 64; ++mb)
+    for (int n0 = 0; n0 < N; n0 += 8) {
+      const Opnd a = TA ? Opnd{{smem_u32(sA) + (uint32_t)mb * 8u * (uint32_t)K * 16u, 0u, 0u}, 256u, 128u, (uint32_t)K * 16u}
+                        : Opnd{{smem_u32(sA) + (uint32_t)mb * 1024u, 0u, 0u}, 2u * (uint32_t)M * 16u, (uint32_t)M * 16u, 128u};
+      const Opnd b = TB ? Opnd{{smem_u32(sB) + (uint32_t)(n0 / 8) * (uint32_t)K * 16u, 0u, 0u}, 256u, 128u, (uint32_t)K * 16u}
+                        : Opnd{{smem_u32(sB) + (uint32_t)n0 * 16u, 0u, 0u}, 2u * (uint32_t)N * 16u, (uint32_t)N * 16u, 128u};
+      float d[4];
+      wg_gemm<8, TA, TB>(d, a, b, 1, K / 16);
+      frag_foreach<8>(d, [&](int r, int c, float x, float y) {
+        C[(size_t)(64 * mb + r) * N + n0 + c] = x;
+        C[(size_t)(64 * mb + r) * N + n0 + c + 1] = y;
+      });
+    }
+}
 __global__ void __launch_bounds__(128) k_tc_selftest2(const unsigned char* __restrict__ A, const unsigned char* __restrict__ B,
                                                       float* __restrict__ C, int M, int N, int K, int a_mn, int b_mn) {
   using namespace l4dtc;
-  extern __shared__ __align__(1024) unsigned char tc_smem[];
-  __shared__ __align__(8) uint64_t bar;
-  __shared__ uint32_t tmem_base_s;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  extern __shared__ __align__(128) unsigned char tc_smem[];
+  const int tid = threadIdx.x;
   const int a_bytes = M * K * 2, b_bytes = N * K * 2;
   unsigned char* sA = tc_smem;
   unsigned char* sB = tc_smem + ((a_bytes + 1023) & ~1023);
-  if (tid == 0) { mbar_init(&bar, 1); fence_mbar_init(); }
-  if (warp == 0) tmem_alloc(&tmem_base_s, 256);
   for (int i = tid * 16; i < a_bytes; i += 128 * 16) *reinterpret_cast<uint4*>(sA + i) = *reinterpret_cast<const uint4*>(A + i);
   for (int i = tid * 16; i < b_bytes; i += 128 * 16) *reinterpret_cast<uint4*>(sB + i) = *reinterpret_cast<const uint4*>(B + i);
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tbase = tmem_base_s;
-  if (tid == 0) {
-    const uint32_t idesc = idesc_f16((uint32_t)M, (uint32_t)N, (uint32_t)a_mn, (uint32_t)b_mn);
-    for (int k = 0; k < K / 16; ++k) {
-      const uint64_t da = a_mn ? smem_desc(smem_u32(sA) + (uint32_t)k * 256u, 128u, (uint32_t)K * 16u)
-                               : smem_desc(smem_u32(sA) + (uint32_t)(2 * k) * (uint32_t)M * 16u, (uint32_t)M * 16u, 128u);
-      const uint64_t db = b_mn ? smem_desc(smem_u32(sB) + (uint32_t)k * 256u, 128u, (uint32_t)K * 16u)
-                               : smem_desc(smem_u32(sB) + (uint32_t)(2 * k) * (uint32_t)N * 16u, (uint32_t)N * 16u, 128u);
-      umma_f16(tbase, da, db, idesc, k > 0 ? 1u : 0u);
-    }
-    umma_commit(&bar);
-  }
-  mbar_wait(&bar, 0);
-  tc_fence_after();
-  // every lane of the warp's sub-partition is read; only lanes that hold a row store it
-  for (int n0 = 0; n0 < N; n0 += 16) {
-    float v[16];
-    tmem_ld16(tbase + ((uint32_t)(warp * 32) << 16) + (uint32_t)n0, v);
-    int row = -1;
-    if (M == 128) row = tid; else if (lane < 16) row = warp * 16 + lane;
-    if (row >= 0) {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) if (n0 + i < N) C[(size_t)row * N + n0 + i] = v[i];
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tbase, 256);
+  if (a_mn && b_mn) tc_selftest2_body<1, 1>(sA, sB, C, M, N, K);
+  else if (a_mn) tc_selftest2_body<1, 0>(sA, sB, C, M, N, K);
+  else if (b_mn) tc_selftest2_body<0, 1>(sA, sB, C, M, N, K);
+  else tc_selftest2_body<0, 0>(sA, sB, C, M, N, K);
 }

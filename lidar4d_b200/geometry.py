@@ -289,7 +289,7 @@ class FieldConfig:
         return hidden * n_in_pad + (n_hidden_layers - 1) * hidden * hidden + n_out_pad * hidden
 
     def validate(self) -> None:
-        """The sm_100a kernels are specialised for the reference defaults that
+        """The sm_90a kernels are specialised for the reference defaults that
         its CLI never changes in the shipped run scripts (run_kitti_lidar4d.sh);
         n_levels_hash / hashmap sizes / resolutions / num_frames stay runtime."""
         assert self.n_features_per_level_hash == 4, "time basis needs F=4 (hash_field.py:38,62)"

@@ -127,7 +127,7 @@ class _Engine:
         self.owner = owner
         self.cfg = cfg if cfg is not None else owner.cfg
         # default = what the reference does: tiny-cuda-nn's FullyFusedMLP consumes fp16 copies of its fp32 parameters;
-        # this is also the mode that runs the dense kernels on the tcgen05 tensor cores
+        # this is also the mode that runs the dense kernels on the wgmma tensor cores
         self.mlp_fp16 = True
         self.ccfg = _capi.make_config(self.cfg, True)
         self.names = _capi.param_names(self.cfg)
@@ -189,7 +189,7 @@ class _Engine:
     def _require_cuda(self, *ts):
         dev = self.device()
         if dev.type != "cuda":
-            raise RuntimeError("lidar4d_b200 runs on CUDA (sm_100a) only; move the model with .cuda() "
+            raise RuntimeError("lidar4d_b200 runs on CUDA (sm_90a) only; move the model with .cuda() "
                                "(there is no CPU fallback)")
         for t in ts:
             if t is not None and t.device != dev:
@@ -629,7 +629,7 @@ class LiDAR4D(LiDAR_Renderer):
     def set_mlp_fp16(self, on: bool = True):
         """True: MLP weights are consumed as fp16-rounded working copies of the fp32 masters (exactly how
         tiny-cuda-nn's FullyFusedMLP holds them) and the dense kernels of the split pipeline run on the
-        tcgen05 tensor cores with hi/lo-split fp16 activations (fp32-class accuracy) -- the default.
+        wgmma tensor cores with hi/lo-split fp16 activations (fp32-class accuracy) -- the default.
         False: fp32 weights on the fp32-FMA kernels (bit-for-bit the fp32 oracle's arithmetic, ~2x slower)."""
         self._engine.set_mlp_fp16(on)
         return self

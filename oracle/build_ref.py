@@ -1,10 +1,10 @@
 """ORACLE support (test infrastructure, NOT product code): compile the reference's OWN chamfer extension
-(/root/reference/utils/chamfer3D/chamfer3D.cu + chamfer_cuda.cpp, a self-contained torch cpp-extension) for sm_100a
+(/root/reference/utils/chamfer3D/chamfer3D.cu + chamfer_cuda.cpp, a self-contained torch cpp-extension) for sm_90a
 from the sources where they lie, into oracle/_ref/ (git-ignored, travels to the GPU box with the snapshot).
 
     python oracle/build_ref.py            # build container only: needs /root/reference (read-only) and nvcc
 
-It is used (a) as the TRUE oracle of tests/test_chamfer.py - distances and indices of the B200 kernel must equal the
+It is used (a) as the TRUE oracle of tests/test_chamfer.py - distances and indices of the CUDA kernel must equal the
 reference kernel's bit for bit - and (b) as the same-box performance bar of the chamfer op (bench.py / profiles).
 Nothing is copied: the two source files are compiled in place by torch.utils.cpp_extension (ninja + nvcc), the
 reference's own setup.py / JIT loader (dist_chamfer_3D.py:8-28) is not run.  The rest of the reference's hot path
@@ -32,10 +32,10 @@ def build(force: bool = False) -> str:
     if os.path.exists(out) and not force and all(os.path.getmtime(s) < os.path.getmtime(out) for s in srcs):
         return out
     os.makedirs(OUT, exist_ok=True)
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     from torch.utils import cpp_extension
     cpp_extension.load(name=NAME, sources=srcs, build_directory=OUT, verbose=True, is_python_module=False,
-                       extra_cuda_cflags=["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo"])
+                       extra_cuda_cflags=["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo"])
     return out
 
 

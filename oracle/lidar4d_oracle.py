@@ -192,7 +192,7 @@ def jitter_uniform(seed: int, ray_index: np.ndarray, n_steps: int) -> np.ndarray
 def sample_lin(n_steps: int) -> np.ndarray:
     """torch.linspace(0,1,S) exactly as the CUDA kernel computes it (the reference renders on the GPU,
     renderer.py:77): step*j below the midpoint, fma(-step, S-1-j, 1) - ONE rounding - above it.  Pinned against the
-    real thing: tests/golden/cuda_linspace.npz was dumped from torch.linspace(device="cuda") on a B200."""
+    real thing: tests/golden/cuda_linspace.npz was dumped from torch.linspace(device="cuda") on a GPU."""
     step = np.float32(1.0) / np.float32(n_steps - 1) if n_steps > 1 else np.float32(0)
     j = np.arange(n_steps)
     lo = (step * j.astype(np.float32)).astype(np.float32)
@@ -512,7 +512,7 @@ def band_limit_tables(model: OracleLiDAR4D) -> OracleLiDAR4D:
     cell size, so every level contributes the same slope).  With the white-noise tables of randomize_parameters one ulp
     (6e-8) of a warped coordinate x + flow moves a 32769-cell level by 2e-3 cells = a 1e-3 feature change: two correct
     fp32 implementations then differ by ~5e-5 in the weights and disagree on ReLU / texel decisions of individual
-    samples, which shows up as per-entry differences of sparse table gradients (measured on the B200:
+    samples, which shows up as per-entry differences of sparse table gradients (observed on a GPU:
     profiles/r02_parity_*).  Band-limited tables keep that amplification at 1 and gradients comparable entry by entry."""
     with torch.no_grad():
         for k, v in model.P.items():

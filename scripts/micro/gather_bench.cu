@@ -25,7 +25,7 @@ __global__ void __launch_bounds__(128) k(const unsigned char* __restrict__ table
 }
 template <int BYTES>
 static double run(const unsigned char* t, uint32_t n_sectors, float* out, int per_sm) {
-  const int blocks = 148 * per_sm, threads = 128, iters = 64;
+  const int blocks = 132 * per_sm, threads = 128, iters = 64;
   cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
   k<BYTES><<<blocks, threads>>>(t, n_sectors, 4, out);
   cudaDeviceSynchronize();

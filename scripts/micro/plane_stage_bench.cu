@@ -73,7 +73,7 @@ typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void
                              const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 template <bool COH>
 static void run(const float* plane, const CUtensorMap& tm, float* out, int per_sm, const char* name, bool first) {
-  const int blocks = 148 * per_sm, threads = 128, iters = 512;
+  const int blocks = 132 * per_sm, threads = 128, iters = 512;
   const size_t smem = PW * PH * PC * 4;
   cudaFuncSetAttribute(k_tma<COH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);

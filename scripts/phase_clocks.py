@@ -30,7 +30,7 @@ lib.l4d_debug_phase_clocks(buf)
 v = np.array(list(buf), dtype=np.float64)
 tot = v.sum()
 n_tiles = N * 6
-print(f"[clk] total {tot/148/1.965e6:.2f} ms per CTA; {tot/n_tiles:.0f} cycles per tile")
+print(f"[clk] total {tot/132/1.98e6:.2f} ms per CTA; {tot/n_tiles:.0f} cycles per tile")
 for i in range(13):
     if v[i] > 0:
         print(f"[clk] {i:2d} {names.get(i,''):34s} {100*v[i]/tot:6.2f}%  {v[i]/n_tiles:9.0f} cyc/tile")

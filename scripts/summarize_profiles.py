@@ -85,7 +85,7 @@ if os.path.exists(rep):
             top = max(pipes, key=pipes.get)
             d["limiter"] = f"{top} = {pipes[top]:.0f} % of peak (ncu --set full, {tag})"
             d["limiter_unit"] = {"l1tex_lsu_data_pipe_pct": "L1TEX LSU data pipe (wavefronts)", "l2_throughput_pct": "L2 (lts) throughput",
-                                 "dram_throughput_pct": "DRAM (HBM) throughput", "tensor_pipe_pct": "tensor pipe (tcgen05)",
+                                 "dram_throughput_pct": "DRAM (HBM) throughput", "tensor_pipe_pct": "tensor pipe",
                                  "fma_pipe_pct": "FP32 FMA pipe"}[top]
             d["limiter_pct"] = pipes[top]
         binding[name] = d

@@ -23,7 +23,7 @@ def build(force=False):
     if not force and os.path.exists(SO) and all(os.path.getmtime(SO) >= os.path.getmtime(d) for d in deps):
         return SO
     cmd = ["nvcc", "-O2", "-std=c++17", "-shared", "-Xcompiler", "-fPIC,-ffp-contract=off",
-           "-gencode", "arch=compute_100a,code=sm_100a", "-o", SO, SRC]
+           "-gencode", "arch=compute_90a,code=sm_90a", "-o", SO, SRC]
     subprocess.run(cmd, check=True)
     return SO
 
@@ -38,7 +38,7 @@ def build_warpsim(force=False):
     if not force and os.path.exists(WS_SO) and all(os.path.getmtime(WS_SO) >= os.path.getmtime(d) for d in deps):
         return WS_SO
     cmd = ["nvcc", "-O2", "-std=c++17", "-shared", "-Xcompiler", "-fPIC,-ffp-contract=off",
-           "-gencode", "arch=compute_100a,code=sm_100a", "-o", WS_SO, WS_SRC, "-lpthread"]
+           "-gencode", "arch=compute_90a,code=sm_90a", "-o", WS_SO, WS_SRC, "-lpthread"]
     subprocess.run(cmd, check=True)
     return WS_SO
 

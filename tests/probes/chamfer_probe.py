@@ -37,9 +37,9 @@ for (n, m) in ((1024, 1024), (30000, 30000), (100000, 100000)):
     fwd = e[0].elapsed_time(e[1]) / reps
     both = e[1].elapsed_time(e[2]) / reps
     pairs = 2.0 * n * m
-    # FP32 pipe: 6 lane-operations per pair (3 subtractions, 1 multiply, 2 fma; packed FADD2/FMUL2/FFMA2 carry two
-    # each) at 128 lanes per clock per SM: 148 SMs x 128 x 1.965 GHz / 6
-    peak_pairs = 148 * 128 * 1.965e9 / 6
+    # FP32 pipe: 6 lane-operations per pair (3 subtractions, 1 multiply, 2 fma) at 128 lanes per clock per SM:
+    # 132 SMs x 128 x 1.98 GHz / 6
+    peak_pairs = 132 * 128 * 1.98e9 / 6
     out[f"{n}x{m}"] = {"fwd_ms": fwd, "fwd_bwd_ms": both, "pairs_per_s": pairs / (fwd * 1e-3),
                        "frac_of_fp32_pipe_peak": pairs / (fwd * 1e-3) / peak_pairs}
     if ref_ext is not None:

@@ -1,7 +1,7 @@
 """SURVEY.md 8(d)(ii): the reference-equivalent PyTorch path in GPU eager mode, timed next to the CUDA path.
 
 The true reference (PyTorch + tiny-cuda-nn) cannot run in this environment; its closest stand-in on a GPU is the
-oracle (the reference's op graph restated in plain torch on the tcnn spec) executed eagerly on the same B200.
+oracle (the reference's op graph restated in plain torch on the tcnn spec) executed eagerly on the same GPU.
 Test infrastructure (lives under tests/, imports oracle/); prints one JSON line."""
 import json, os, sys
 import numpy as np, torch

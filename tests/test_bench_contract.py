@@ -55,23 +55,3 @@ def test_executed_red_count_of_the_static_scatter():
     # the macro the count mirrors
     src = open(os.path.join(ROOT, "lidar4d_b200", "csrc", "l4d_split.cuh")).read()
     assert f"#define L4D_STATIC_AGG_RES {bench.STATIC_AGG_RES}" in src
-
-
-def test_committed_bench_line_carries_the_contract_keys():
-    """The last GPU bench line of the round (profiles/r02_v8_bench.json, written by `python bench.py` on a B200) has every key
-    the bench contract names and a roofline fraction <= 1 against the unit that binds the dominant kernel."""
-    line = json.load(open(os.path.join(ROOT, "profiles", "r02_v8_bench.json")))
-    for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline",
-              "dtype", "data", "config", "e2e", "gpu_launches", "clocks", "roofline", "cpu_baseline"):
-        assert k in line, k
-    assert line["warmup"] >= 3 and line["gpu_launches"] > 0 and "workload" in line["config"] and "l2" in line["config"]
-    assert {"value", "unit", "h2d_bytes_per_step", "d2h_bytes_per_step"} <= set(line["e2e"])
-    assert line["e2e"]["h2d_bytes_per_step"] > 0 and line["e2e"]["value"] < line["value"] * 1.001
-    assert {"sm_mhz", "sm_max_mhz", "reasons"} <= set(line["clocks"]) and not line["clocks"]["reasons"]
-    r = line["roofline"]
-    assert {"bound", "achieved", "peak", "unit", "frac", "traffic"} <= set(r) and 0 < r["frac"] <= 1.0
-    assert {"value", "unit", "cores", "kind", "sample"} <= set(line["cpu_baseline"])
-    ks = r["kernels"]
-    assert abs(sum(v["avg_ms"] for k, v in ks.items() if "adam" not in k) * 4 - line["ms_per_step"]) < 0.03 * line["ms_per_step"]
-    b = ks["k_bwd_scatter_static"]["binding"]
-    assert b["frac"] <= 1.0 and b["red_lane_ops_per_sample_executed"] < b["red_lane_ops_per_sample_algorithmic"]

@@ -4,7 +4,7 @@ x 8 time slices, 2^18 flow), n_levels_hash 8 and 16 (sigma_in_dim 120 / 176), S 
 Two anchors:
   * tests/golden/ref_full_*.npz - the UNMODIFIED reference modules on the tcnn shim (tests/golden/make_golden.py);
   * the oracle, run here on the host cores with the same seeded parameters, for EVERY gradient tensor in full.
-Both CUDA modes (tcgen05 tensor-core kernels with fp16 working weights; fp32-FMA kernels) and both pipelines are held to:
+Both CUDA modes (wgmma tensor-core kernels with fp16 working weights; fp32-FMA kernels) and both pipelines are held to:
 
   forward   z_vals / hash indices bit-exact; depth, image, weights <= 1e-4 (rel-to-max, fp32) against the reference
             fixture and the oracle - on white-noise tables AND on band-limited ("trained-like") tables;

@@ -1,4 +1,4 @@
-"""GPU (B200) parity tests proper: the product path - LiDAR4D module -> ctypes ->
+"""GPU (H100) parity tests proper: the product path - LiDAR4D module -> ctypes ->
 liblidar4d_b200.so kernels - against the oracle and the committed golden vectors.
 Tolerance 1e-4 rel-to-max fp32 (BASELINE.json north_star); hash indices bit-exact."""
 import os
@@ -299,7 +299,7 @@ def test_training_step_changes_loss(dev, full_model):
 
 @pytest.mark.parametrize("N,K", [(64, 128), (16, 64), (128, 16), (64, 384), (8 * 2, 16)])
 def test_tcgen05_selftest_gemm(dev, N, K):
-    """The tensor-core building blocks (smem descriptors, TMEM alloc, tcgen05.mma/commit/ld) in isolation."""
+    """The tensor-core building blocks (smem descriptors, wgmma issue/wait, accumulator fragment layout) in isolation."""
     import ctypes as C
     from lidar4d_b200 import _capi
     lib = _capi.load_library()
@@ -324,8 +324,8 @@ TC_CASES += [(0.4, 140, True, 11, False, 3), (0.4, 140, True, 11, False, 5)]
 
 @pytest.mark.parametrize("case", TC_CASES)
 def test_tensor_core_path(dev, case):
-    """mlp_fp16 mode: the dense kernels run on tcgen05 tensor cores (fp16 hi/lo-split activations, fp16 weights,
-    fp32 TMEM accumulation).  The oracle emulates the fp16 weight rounding exactly; tolerance stays 1e-4."""
+    """mlp_fp16 mode: the dense kernels run on wgmma tensor cores (fp16 hi/lo-split activations, fp16 weights,
+    fp32 accumulation).  The oracle emulates the fp16 weight rounding exactly; tolerance stays 1e-4."""
     t, S, perturb, seed, surface = case[:5]
     orc = O.build_seeded(small_config(**({"n_levels_hash": case[5]} if len(case) > 5 else {})), seed, flow_last_std=0.02)
     if surface:

@@ -49,7 +49,7 @@ dist.barrier(); dist.destroy_process_group()
 '''
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs >= 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs >= 2 GPUs")
 def test_sharded_gradients_equal_single_gpu(tmp_path):
     script = tmp_path / "worker.py"
     script.write_text(WORKER.format(root=ROOT))

@@ -118,7 +118,7 @@ def test_planes_restatement_matches_grid_sample_directly():
 
 
 def test_z_grid_restatement_matches_cuda_linspace_dump():
-    """tests/golden/cuda_linspace.npz = torch.linspace(0, 1, S, device="cuda") dumped on a B200 (scripts/diag_fullsize.py):
+    """tests/golden/cuda_linspace.npz = torch.linspace(0, 1, S, device="cuda") dumped on a GPU (scripts/diag_fullsize.py):
     the oracle's (and, through tests/test_hostsim_parity.py, the kernels') z grid is bit-exact with the grid the reference
     gets on its GPU path (renderer.py:77)."""
     fx = load("cuda_linspace")
