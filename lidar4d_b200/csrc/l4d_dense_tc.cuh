@@ -1,14 +1,14 @@
 // l4d_dense_tc.cuh - tensor-core (wgmma) versions of the dense kernels of the split pipeline.
 // Requires mlp_fp16 (MLP weights are fp16 working copies, as tiny-cuda-nn keeps them).
 //
-// Tile = 128 samples; in the epilogues thread (threadIdx.x % 128) owns sample row.
+// Tile = 128 samples; warpgroup w owns rows [64w, 64w + 64) of every product.
 // Operands live in shared memory as fp16 in the K-major interleaved layout of l4d_tc.cuh
 // ([k/8][row][8 halves], 16-byte chunks).  Activations are carried as hi + lo fp16 pairs
 // (x = hi + lo to ~2^-22 relative), i.e. every product with an fp16 weight is exact and the fp32
 // accumulation reproduces the fp32-FMA kernels to ~1e-6: the 1e-4 parity bar holds on the
-// tensor-core path too.  Every warpgroup issues the wgmma of its 64-row block; activation products
-// go through the fp32 staging tile (one row per thread), weight gradients are flushed with fp32
-// atomics straight from the accumulator registers.
+// tensor-core path too.  Every warpgroup issues the wgmma of its 64-row block and runs the epilogues
+// on the accumulator fragments in its registers; weight gradients are flushed with fp32 atomics
+// straight from there.
 #pragma once
 #include "l4d_core.cuh"
 #include "l4d_tc.cuh"
@@ -43,38 +43,70 @@ __device__ __forceinline__ void publish() {
   __syncthreads();
 }
 
-// The products below are called by every thread of the CTA; the warpgroups split the two 64-row blocks of a
-// 128-sample product.  A thread may read the staging tile only after the __syncthreads() that follows.
+// warpgroup-wide: make this warpgroup's generic-proxy tile writes visible to its own next wgmma
+__device__ __forceinline__ void wg_publish() {
+  fence_proxy_async();
+  wg_bar();
+}
+
+// The products below are warpgroup-wide and cover the 64-row block [m0, m0 + 64) of a 128-row tile; the result stays
+// in the caller's registers (fragment layout of l4d_tc.cuh).
 //
-// D[128 x N] = (Ah + Al) * B^T over n_chunks 16-byte k-chunks (n_chunks even): A = 128-row tiles (chunk stride 2048),
-// B = K-major [k/8][b_rows][8] (b points at its first used row) -> staging columns [c0, c0 + N)
+// D[64 x N] = (Ah + Al) * B^T over n_chunks 16-byte k-chunks (n_chunks even): A = 128-row tiles (chunk stride 2048),
+// B = K-major [k/8][b_rows][8] (b points at its first used row)
 template <int N>
-__device__ __forceinline__ void mma_rows(float* S, int c0, uint32_t a_hi, uint32_t a_lo, uint32_t b, uint32_t b_rows, int n_chunks) {
-  for (int mb = threadIdx.x >> 7; mb < 2; mb += blockDim.x >> 7) {
-    const Opnd a{{a_hi + (uint32_t)mb * 1024u, a_lo + (uint32_t)mb * 1024u, 0u}, 4096u, 2048u, 128u};
-    const Opnd w{{b, b, 0u}, 2u * b_rows * 16u, b_rows * 16u, 128u};
-    float d[N / 2];
-    wg_gemm<N, 0, 0>(d, a, w, 2, n_chunks / 2);
-    acc_store<N>(S, d, 64 * mb, c0);
-  }
+__device__ __forceinline__ void mma_rows(float (&d)[N / 2], int m0, uint32_t a_hi, uint32_t a_lo, uint32_t b, uint32_t b_rows, int n_chunks) {
+  const Opnd a{{a_hi + (uint32_t)m0 * 16u, a_lo + (uint32_t)m0 * 16u, 0u}, 4096u, 2048u, 128u};
+  const Opnd w{{b, b, 0u}, 2u * b_rows * 16u, b_rows * 16u, 128u};
+  wg_gemm<N, 0, 0>(d, a, w, 2, n_chunks / 2);
 }
-// D[128 x N] = (Ah + Al) * W: W stored [k_in/8][w_rows][8] (forward layout) and read as B(n = k_in, k = row), i.e.
-// MN-major; w points at the chunk of the first k_in column used.  f(row, col, v[col], v[col + 1]) per element pair.
-template <int N, class F>
-__device__ __forceinline__ void mma_prop_frag(uint32_t a_hi, uint32_t a_lo, int n_chunks, uint32_t w, uint32_t w_rows, F&& f) {
-  for (int mb = threadIdx.x >> 7; mb < 2; mb += blockDim.x >> 7) {
-    const Opnd a{{a_hi + (uint32_t)mb * 1024u, a_lo + (uint32_t)mb * 1024u, 0u}, 4096u, 2048u, 128u};
-    const Opnd b{{w, w, 0u}, 256u, 128u, w_rows * 16u};
-    float d[N / 2];
-    wg_gemm<N, 0, 1>(d, a, b, 2, n_chunks / 2);
-    frag_foreach<N>(d, [&](int r, int c, float x, float y) { f(64 * mb + r, c, x, y); });
-  }
+// D[64 x N] = (Ah + Al) * W: W stored [k_in/8][w_rows][8] (forward layout) and read as B(n = k_in, k = row), i.e.
+// MN-major; w points at the chunk of the first k_in column used.  Issued as one wgmma group; the caller waits.
+template <int N>
+__device__ __forceinline__ void mma_prop_issue(float (&d)[N / 2], int m0, uint32_t a_hi, uint32_t a_lo, int n_chunks, uint32_t w, uint32_t w_rows) {
+  const Opnd a{{a_hi + (uint32_t)m0 * 16u, a_lo + (uint32_t)m0 * 16u, 0u}, 4096u, 2048u, 128u};
+  const Opnd b{{w, w, 0u}, 256u, 128u, w_rows * 16u};
+  wg_gemm_issue<N, 0, 1>(d, a, b, 2, n_chunks / 2);
 }
 template <int N>
-__device__ __forceinline__ void mma_prop(float* S, int c0, uint32_t a_hi, uint32_t a_lo, int n_chunks, uint32_t w, uint32_t w_rows) {
-  mma_prop_frag<N>(a_hi, a_lo, n_chunks, w, w_rows, [&](int r, int c, float x, float y) {
-    *reinterpret_cast<float2*>(S + acc_idx(r, c0 + c)) = make_float2(x, y);
-  });
+__device__ __forceinline__ void mma_prop(float (&d)[N / 2], int m0, uint32_t a_hi, uint32_t a_lo, int n_chunks, uint32_t w, uint32_t w_rows) {
+  mma_prop_issue<N>(d, m0, a_hi, a_lo, n_chunks, w, w_rows);
+  wg_wait<0>();
+}
+// v = relu(d); bit i of the result = element d[i] was positive.  The epilogues of the dense kernels write their results
+// to a separate array: a non-wgmma write to an accumulator makes ptxas serialize every wgmma of the kernel.
+template <int N>
+__device__ __forceinline__ uint32_t frag_relu(const float (&d)[N / 2], float (&v)[N / 2]) {
+  uint32_t m = 0u;
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) {
+    const bool on = d[i] > 0.f;
+    v[i] = on ? d[i] : 0.f;
+    m |= on ? (1u << i) : 0u;
+  }
+  return m;
+}
+// column c of a 64 x 16 fragment (rows [m0, m0 + 64)) -> column c + SHIFT of a 16-wide 128-row hi|lo tile; columns that
+// land outside [0, 16) are dropped.  Rounding as tile_put8.
+template <int SHIFT>
+__device__ __forceinline__ void frag_put16_shift(unsigned char* hi, unsigned char* lo, int m0, const float (&d)[8]) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int c = 8 * (i >> 2) + frag_col() + (i & 1) + SHIFT, r = m0 + frag_row() + 8 * ((i >> 1) & 1);
+    if (c < 0 || c > 15) continue;
+    const __half x = __float2half_rn(d[i]);
+    const __half y = __float2half_rn(d[i] - __half2float(x));
+    const size_t off = ((size_t)(c >> 3) * 128 + r) * 16 + (c & 7) * 2;
+    *reinterpret_cast<__half*>(hi + off) = x;
+    *reinterpret_cast<__half*>(lo + off) = y;
+  }
+}
+// one fp16 element (row r, column c) of a 128-row hi|lo tile
+__device__ __forceinline__ void tile_put1(unsigned char* hi, unsigned char* lo, int r, int c, float v) {
+  const __half x = __float2half_rn(v);
+  const size_t off = ((size_t)(c >> 3) * 128 + r) * 16 + (c & 7) * 2;
+  *reinterpret_cast<__half*>(hi + off) = x;
+  *reinterpret_cast<__half*>(lo + off) = __float2half_rn(v - __half2float(x));
 }
 
 }  // namespace l4dtc
@@ -85,8 +117,7 @@ struct DenseFwdSmem {
   uint32_t xh, xl;                  // feature tile (later reused for the 128-wide attribute hidden tile)
   uint32_t hh, hl;                  // 64-wide hidden tile
   uint32_t gh, gl;                  // 16-wide tile (geo)
-  uint32_t misc;                    // enc[80] cdir[128] w[32] floats
-  uint32_t acc;                     // fp32 staging tile
+  uint32_t misc;                    // enc[80] cdir[128] w[32] sig[128] att[2][128] floats
   uint32_t total;
 };
 __host__ __device__ inline DenseFwdSmem dense_fwd_smem(uint32_t in_pad) {
@@ -99,8 +130,7 @@ __host__ __device__ inline DenseFwdSmem dense_fwd_smem(uint32_t in_pad) {
   L.xh = take(xbytes); L.xl = take(xbytes);
   L.hh = take(64 * 128 * 2); L.hl = take(64 * 128 * 2);
   L.gh = take(16 * 128 * 2); L.gl = take(16 * 128 * 2);
-  L.misc = take((80 + 128 + 32) * 4);
-  L.acc = take(l4dtc::acc_tile_bytes());
+  L.misc = take((80 + 128 + 32 + 128 + 256) * 4);
   L.total = o;
   return L;
 }
@@ -117,7 +147,7 @@ __host__ __device__ inline DenseFwdSmem dense_fwd_smem(uint32_t in_pad) {
 // loss-scaled or tiny upstream gradients neither overflow nor flush; the scale is undone when the
 // fp32 accumulators are read back.  Weight-gradient accumulators are flushed from the registers with fp32
 // atomics once per tile (same count as the FMA kernel's tile_outer_accum).
-// Shared memory at sigma_in_pad = 176 (L = 16): 226 KB, within the 227 KB an sm_90 CTA may use; one CTA per SM.
+// Shared memory at sigma_in_pad = 176 (L = 16): 196 KB; one CTA per SM.
 // =============================================================================================
 struct DenseBwdSmem {
   uint32_t w1, w2, wa1[2], wa2[2];
@@ -125,7 +155,6 @@ struct DenseBwdSmem {
   uint32_t RH;           // 32 KB: sigma hidden hi|lo, later its delta
   uint32_t g16, do16, do8;   // small tiles, hi|lo
   uint32_t misc;
-  uint32_t acc;          // 32 KB fp32 staging tile
   uint32_t total;
 };
 __host__ __device__ inline DenseBwdSmem dense_bwd_smem(uint32_t in_pad) {
@@ -137,8 +166,7 @@ __host__ __device__ inline DenseBwdSmem dense_bwd_smem(uint32_t in_pad) {
   L.wa2[0] = take(64 * 64 * 2); L.wa2[1] = take(64 * 64 * 2);
   L.R = take(96 * 1024); L.RH = take(32 * 1024);
   L.g16 = take(2 * 4096); L.do16 = take(2 * 4096); L.do8 = take(2 * 2048);
-  L.misc = take((80 + 128 + 128 + 128 + 32 + 64) * 4);
-  L.acc = take(l4dtc::acc_tile_bytes());
+  L.misc = take((80 + 128 + 128 + 128 + 32 + 64 + 128 + 256 + 128) * 4);
   L.total = o;
   return L;
 }
@@ -237,9 +265,10 @@ __device__ __forceinline__ float block_amax256(float v, float* s_w) {
 }  // namespace l4dtc
 
 // -------------------------------------------------------------------------------------------
-// forward 2/2 on tensor cores: sigma MLP, compositing, attribute heads.  One CTA per ray, 256 threads: two threads per
-// row (sample) split the columns of every epilogue; in the attribute phase thread half h owns head h, and the heads'
-// products pass through the 64-column staging tile one after the other.
+// forward 2/2 on tensor cores: sigma MLP, compositing, attribute heads.  One CTA per ray, 256 threads: warpgroup w
+// computes rows [64w, 64w + 64) of every product and runs its epilogues on the accumulator fragments; the compositing
+// scans run in row order (two threads per row, thread half h accumulates head h) and exchange per-row values with the
+// fragments through small per-row arrays.
 // -------------------------------------------------------------------------------------------
 namespace l4dtc {
 // sum over the 128 rows of one thread half (warps 0-3 / 4-7) of a 256-thread CTA; every thread of the half gets it
@@ -268,7 +297,9 @@ __global__ void __launch_bounds__(256) k_fwd_dense_tc(const __grid_constant__ Sp
   float* s_enc = reinterpret_cast<float*>(dsm + L.misc);
   float* s_cdir = s_enc + 80;
   float* s_w = s_cdir + 128;
-  float* S = reinterpret_cast<float*>(dsm + L.acc);
+  float* s_sig = s_w + 32;         // per row: sigma pre-activation (output column 0)
+  float* s_att = s_sig + 128;      // per head and row: attribute logit
+  const int m0 = 64 * half;        // rows of this warpgroup
   const uint32_t sb = smem_u32(dsm);
 
   if (tid == 0) { mbar_init(&s_xbar, 1); fence_mbar_init(); }
@@ -334,27 +365,25 @@ __global__ void __launch_bounds__(256) k_fwd_dense_tc(const __grid_constant__ Sp
       mbar_wait(&s_xbar, xphase);      // this tile's features have landed
       xphase ^= 1u;
       publish();
-      mma_rows<64>(S, 0, sb + L.xh, sb + L.xl, sb + L.w1, 64, n_xchunks);
-      __syncthreads();
-      // ---- hidden = relu(.) -> hi/lo tile (each half its 32 columns) ----
-#pragma unroll
-      for (int qq = 0; qq < 2; ++qq) {
-        const int q = 2 * half + qq;
-        float v[16];
-        acc_ld16(S, q * 16, v);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i], 0.f);
-        tile_put8(hh, hl, row, 2 * q, v);
-        tile_put8(hh, hl, row, 2 * q + 1, v + 8);
+      // ---- warpgroup wg: rows [m0, m0 + 64).  hidden = relu(X W1^T) -> hi/lo tile, then the output layer ----
+      {
+        float d[32];
+        mma_rows<64>(d, m0, sb + L.xh, sb + L.xl, sb + L.w1, 64, n_xchunks);
+        float v[32];
+        frag_relu<64>(d, v);
+        frag_put<64>(hh, hl, 128, m0, 0, v);
       }
-      publish();
-      mma_rows<16>(S, 0, sb + L.hh, sb + L.hl, sb + L.w2, 16, 8);
+      wg_publish();
+      {
+        float o[8];
+        mma_rows<16>(o, m0, sb + L.hh, sb + L.hl, sb + L.w2, 16, 8);
+        if ((tid & 3) == 0) { s_sig[m0 + frag_row()] = o[0]; s_sig[m0 + frag_row() + 8] = o[2]; }
+        frag_put16_shift<-1>(gh, gl, m0, o);          // geo -> attribute input columns 0..14 (rows outside the mask: below)
+      }
       __syncthreads();
-      float out[16];
-      acc_ld16(S, 0, out);
       float zj = 0.f, alpha = 0.f, sigma = 0.f;
       if (valid) {
-        sigma = expf(out[0]);
+        sigma = expf(s_sig[row]);
         zj = l4d_z(rs, rg, j);
         const float delta = (j + 1 < n_steps) ? (l4d_z(rs, rg, j + 1) - zj) : rs.sample_dist;
         alpha = l4d_alpha(M, delta, sigma);
@@ -370,52 +399,43 @@ __global__ void __launch_bounds__(256) k_fwd_dense_tc(const __grid_constant__ Sp
       if (!any_masked) x_issue_next(ray, j0 >> 7);       // the X buffer is free already
       if (any_masked) {
         // ---- attribute heads: [geo,0] (K=16) -> 2x64 -> relu -> 64 -> relu -> dot w3 -> sigmoid ----
-        {
-          float g8[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float gv = half ? (i < 7 ? out[9 + i] : 0.f) : out[1 + i];      // geo[0..7] | geo[8..14], 0
-            g8[i] = masked ? gv : 0.f;
+        if (half == 0) {
+          if (masked) tile_put1(gh, gl, row, 15, 0.f);
+          else {
+            *reinterpret_cast<uint4*>(tile_chunk(gh, row, 0)) = make_uint4(0u, 0u, 0u, 0u);
+            *reinterpret_cast<uint4*>(tile_chunk(gh, row, 1)) = make_uint4(0u, 0u, 0u, 0u);
+            *reinterpret_cast<uint4*>(tile_chunk(gl, row, 0)) = make_uint4(0u, 0u, 0u, 0u);
+            *reinterpret_cast<uint4*>(tile_chunk(gl, row, 1)) = make_uint4(0u, 0u, 0u, 0u);
           }
-          tile_put8(gh, gl, row, half, g8);
         }
         publish();
 #pragma unroll 1
         for (int net = 0; net < 2; ++net) {    // 128 columns: net0 hidden | net1 hidden -> chunks 0..15 of the x tile
-          mma_rows<64>(S, 0, sb + L.gh, sb + L.gl, sb + L.wa1 + (uint32_t)net * 64u * 16u, 128, 2);
-          __syncthreads();
-          if (half == net) {
+          float d[32];
+          mma_rows<64>(d, m0, sb + L.gh, sb + L.gl, sb + L.wa1 + (uint32_t)net * 64u * 16u, 128, 2);
+          float v[32];
 #pragma unroll
-            for (int qq = 0; qq < 4; ++qq) {
-              const int q = 4 * half + qq;
-              float v[16];
-              acc_ld16(S, qq * 16, v);
-#pragma unroll
-              for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i] + s_cdir[q * 16 + i], 0.f);
-              tile_put8(xh, xl, row, 2 * q, v);
-              tile_put8(xh, xl, row, 2 * q + 1, v + 8);
-            }
-          }
-          publish();
+          for (int i = 0; i < 32; ++i) v[i] = fmaxf(d[i] + s_cdir[net * 64 + 8 * (i >> 2) + frag_col() + (i & 1)], 0.f);
+          frag_put<64>(xh, xl, 128, m0, 8 * net, v);
         }
-        float o = 0.f;
+        wg_publish();
 #pragma unroll 1
         for (int net = 0; net < 2; ++net) {
-          mma_rows<64>(S, 0, sb + L.xh + (uint32_t)net * 8u * 2048u, sb + L.xl + (uint32_t)net * 8u * 2048u, sb + L.wa2[net], 64, 8);
-          __syncthreads();
-          if (half == net) {
+          float d[32];
+          mma_rows<64>(d, m0, sb + L.xh + (uint32_t)net * 8u * 2048u, sb + L.xl + (uint32_t)net * 8u * 2048u, sb + L.wa2[net], 64, 8);
+          float o[2] = {0.f, 0.f};
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              float v[16];
-              acc_ld16(S, q * 16, v);
-#pragma unroll
-              for (int i = 0; i < 16; ++i) o = fmaf(fmaxf(v[i], 0.f), l4d_ld1(M.att_w3[half] + q * 16 + i), o);
-            }
+          for (int i = 0; i < 32; ++i) {
+            const int h = (i >> 1) & 1;
+            o[h] = fmaf(fmaxf(d[i], 0.f), l4d_ld1(M.att_w3[net] + 8 * (i >> 2) + frag_col() + (i & 1)), o[h]);
           }
-          __syncthreads();
+          o[0] = quad_sum(o[0]);
+          o[1] = quad_sum(o[1]);
+          if ((tid & 3) == 0) { s_att[net * 128 + m0 + frag_row()] = o[0]; s_att[net * 128 + m0 + frag_row() + 8] = o[1]; }
         }
+        __syncthreads();
         x_issue_next(ray, j0 >> 7);                    // the attribute hidden tile (in the X buffer) has been consumed
-        if (masked) a = l4d_sigmoid(o);
+        if (masked) a = l4d_sigmoid(s_att[half * 128 + row]);
       }
       pa = fmaf(w, a, pa);
       if (half == 0) { pd = fmaf(w, zj, pd); pw += w; }
@@ -429,7 +449,7 @@ __global__ void __launch_bounds__(256) k_fwd_dense_tc(const __grid_constant__ Sp
           if (A.zvals) A.zvals[p] = zj;
         }
       }
-      __syncthreads();          // the staging tile and the operand tiles are reused by the next tile
+      __syncthreads();          // the operand tiles and the per-row arrays are reused by the next tile
     }
     pd = half_sum(pd, s_w); pa = half_sum(pa, s_w); pw = half_sum(pw, s_w);
     if (tid == 0) { A.depth[ray] = pd; A.image[2 * ray] = pa; A.wsum[ray] = pw; }
@@ -444,8 +464,10 @@ __device__ unsigned long long g_phase_clk[32];
 #define L4D_PH(i) do { } while (0)
 #endif
 
-// 256 threads, two threads per row that split the columns of every epilogue: twice the warps to hide latency, and one
-// warpgroup per 64-row block of every 128-sample product.
+// 256 threads: warpgroup w computes rows [64w, 64w + 64) of every row-wise product and runs its epilogues on the
+// fragments; the compositing scans run in row order (two threads per row) and hand their per-row results to the
+// fragments through small per-row arrays.  The per-tile gradient scales and the weight-gradient products (K = 128
+// samples) still couple the two warpgroups at every delta tile.
 __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ SplitArgs A) {
   using namespace l4dtc;
   extern __shared__ __align__(128) unsigned char dsm[];
@@ -453,7 +475,7 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
   const DevModel& M = A.M;
   const DevGrads& G = A.G;
   const int tid = threadIdx.x;
-  const int row = tid & 127, half = tid >> 7;     // two threads per row: `half` owns columns [32*half, 32*half+32) of every 64-wide block
+  const int row = tid & 127, half = tid >> 7;     // row-order work: two threads per row
   const int wg = half;                            // warpgroup
   const uint32_t in_pad = M.sigma_in_pad;
   const DenseBwdSmem L = dense_bwd_smem(in_pad);
@@ -478,9 +500,10 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
   float* s_csum = s_cdir2 + 128;
   float* s_w = s_csum + 128;
   float* s_tstart = s_w + 32;
-  float* S = reinterpret_cast<float*>(dsm + L.acc);
-  // the attribute phase's per-row dot-product exchange lives in the dO8 tile, which is dead while it is used
-  float* s_part = reinterpret_cast<float*>(o8h);
+  float* s_dsig = s_tstart + 64;   // per row: dL/dsigma, attribute deltas of both heads, attribute mask (0 / 1)
+  float* s_da = s_dsig + 128;
+  float* s_mk = s_da + 256;
+  const int m0 = 64 * wg;          // rows of this warpgroup
   __shared__ float s_w3max[2];
 #ifdef L4D_PHASE_CLOCKS
   __shared__ unsigned long long s_clk[32];
@@ -596,117 +619,94 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
           if (masked) { da[0] = w * gi0; da[1] = w * gi1; }
         }
       }
+      if (half == 0) {      // per-row values for the fragment epilogues (visible after the barrier in publish below)
+        s_dsig[row] = dsigma;
+        s_da[row] = da[0];
+        s_da[128 + row] = da[1];
+        s_mk[row] = masked ? 1.f : 0.f;
+      }
+      // this thread's fragment rows: m0 + frag_row() + 8h
+      const int fr = m0 + frag_row();
 
       L4D_PH(1);
-      // ---------------- P1: sigma MLP forward ----------------
+      // ---------------- P1: sigma MLP forward (rows [m0, m0 + 64) on this warpgroup) ----------------
       x_wait();
       publish();
       L4D_PH(2);
-      mma_rows<64>(S, 0, aXh, aXl, sb + L.w1, 64, n_xchunks);
-      __syncthreads();
-      uint32_t msk = 0u;                       // relu pattern of this half's 32 hidden units
-#pragma unroll
-      for (int qq = 0; qq < 2; ++qq) {
-        const int q = 2 * half + qq;
-        float v[16];
-        acc_ld16(S, q * 16, v);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const bool on = v[i] > 0.f;
-          v[i] = on ? v[i] : 0.f;
-          msk |= on ? (1u << (qq * 16 + i)) : 0u;
-        }
-        tile_put8(hh, hl, row, 2 * q, v);
-        tile_put8(hh, hl, row, 2 * q + 1, v + 8);
+      uint32_t msk;                            // relu pattern of the hidden fragment
+      {
+        float d[32];
+        mma_rows<64>(d, m0, aXh, aXl, sb + L.w1, 64, n_xchunks);
+        float v[32];
+        msk = frag_relu<64>(d, v);
+        frag_put<64>(hh, hl, 128, m0, 0, v);
       }
-      publish();
-      mma_rows<16>(S, 0, aHh, aHl, sb + L.w2, 16, 8);
-      __syncthreads();
-      float out[16], dgeo[16];
-      acc_ld16(S, 0, out);
+      wg_publish();
+      float out[8], dgeo[8];                   // output-layer fragment; dG fragment (geo columns 0..14)
+      mma_rows<16>(out, m0, aHh, aHl, sb + L.w2, 16, 8);
 #pragma unroll
-      for (int i = 0; i < 16; ++i) dgeo[i] = 0.f;
+      for (int i = 0; i < 8; ++i) dgeo[i] = 0.f;
 
       L4D_PH(3);
       // ---------------- P2: attribute heads ----------------
       bool x_dirty = false;          // the attribute phase reuses the X buffer for its tiles
       if (__syncthreads_or(masked ? 1 : 0)) {
-        {   // [geo, 1] tile (zero rows for samples outside the attribute mask)
-          float g[16];
-#pragma unroll
-          for (int i = 0; i < 15; ++i) g[i] = masked ? out[1 + i] : 0.f;
-          g[15] = masked ? 1.0f : 0.f;
-          float g8[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) g8[i] = half ? g[8 + i] : g[i];
-          tile_put8(g16h, g16l, row, half, g8);
+        // [geo, 1] tile, zero rows for samples outside the attribute mask: geo from the fragment, then the row fix-up
+        frag_put16_shift<-1>(g16h, g16l, m0, out);
+        __syncthreads();
+        if (half == 0) {
+          if (masked) tile_put1(g16h, g16l, row, 15, 1.0f);
+          else {
+            *reinterpret_cast<uint4*>(tile_chunk(g16h, row, 0)) = make_uint4(0u, 0u, 0u, 0u);
+            *reinterpret_cast<uint4*>(tile_chunk(g16h, row, 1)) = make_uint4(0u, 0u, 0u, 0u);
+            *reinterpret_cast<uint4*>(tile_chunk(g16l, row, 0)) = make_uint4(0u, 0u, 0u, 0u);
+            *reinterpret_cast<uint4*>(tile_chunk(g16l, row, 1)) = make_uint4(0u, 0u, 0u, 0u);
+          }
         }
+        const bool mk[2] = {s_mk[fr] != 0.f, s_mk[fr + 8] != 0.f};
 #pragma unroll 1
         for (int net = 0; net < 2; ++net) {
-          if (block_amax256(da[net], s_w) == 0.f) continue;       // no gradient reaches this head in this tile
+          if (!__syncthreads_or(da[net] != 0.f ? 1 : 0)) continue;       // no gradient reaches this head in this tile
           x_dirty = true;
           publish();
-          mma_rows<64>(S, 0, aG16h, aG16l, sb + L.wa1[net], 64, 2);
-          __syncthreads();
-          uint32_t m1 = 0u;
+          float d[32], v[32];
+          mma_rows<64>(d, m0, aG16h, aG16l, sb + L.wa1[net], 64, 2);
 #pragma unroll
-          for (int qq = 0; qq < 2; ++qq) {
-            const int q = 2 * half + qq;
-            float v[16];
-            acc_ld16(S, q * 16, v);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float y = v[i] + s_cdir2[net * 64 + q * 16 + i];
-              const bool on = y > 0.f;
-              v[i] = on ? y : 0.f;
-              m1 |= on ? (1u << (qq * 16 + i)) : 0u;
-            }
-            tile_put8(t1h, t1l, row, 2 * q, v);
-            tile_put8(t1h, t1l, row, 2 * q + 1, v + 8);
-          }
-          publish();
-          mma_rows<64>(S, 0, aT1h, aT1l, sb + L.wa2[net], 64, 8);
-          __syncthreads();
+          for (int i = 0; i < 32; ++i) v[i] = d[i] + s_cdir2[net * 64 + 8 * (i >> 2) + frag_col() + (i & 1)];
+          const uint32_t m1 = frag_relu<64>(v, v);
+          frag_put<64>(t1h, t1l, 128, m0, 0, v);
+          wg_publish();
+          mma_rows<64>(d, m0, aT1h, aT1l, sb + L.wa2[net], 64, 8);
+          const uint32_t m2 = frag_relu<64>(d, v);
           float cs = 1.0f;
+          float d_o[2];
           {   // output layer (fp32), sigmoid backward, delta of the second hidden layer
-            float o = 0.f;
-            uint32_t m2 = 0u;
+            float o[2] = {0.f, 0.f};
 #pragma unroll
-            for (int qq = 0; qq < 2; ++qq) {
-              const int q = 2 * half + qq;
-              float v[16];
-              acc_ld16(S, q * 16, v);
+            for (int i = 0; i < 32; ++i)
+              o[(i >> 1) & 1] = fmaf(v[i], l4d_ld1(M.att_w3[net] + 8 * (i >> 2) + frag_col() + (i & 1)), o[(i >> 1) & 1]);
+            frag_put<64>(t2h, t2l, 128, m0, 0, v);
+            float d_raw[2];
 #pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                const bool on = v[i] > 0.f;
-                v[i] = on ? v[i] : 0.f;
-                m2 |= on ? (1u << (qq * 16 + i)) : 0u;
-                o = fmaf(v[i], l4d_ld1(M.att_w3[net] + q * 16 + i), o);
-              }
-              tile_put8(t2h, t2l, row, 2 * q, v);
-              tile_put8(t2h, t2l, row, 2 * q + 1, v + 8);
+            for (int h = 0; h < 2; ++h) {
+              const float a = l4d_sigmoid(quad_sum(o[h]));
+              d_raw[h] = mk[h] ? s_da[net * 128 + fr + 8 * h] * a * (1.0f - a) : 0.f;
             }
-            s_part[half * 128 + row] = o;           // the two halves of the row exchange their partial dot products
-            __syncthreads();
-            o = s_part[row] + s_part[128 + row];
-            const float a = l4d_sigmoid(o);
-            const float d_raw = masked ? da[net] * a * (1.0f - a) : 0.f;
             // per-tile power-of-two scale of the delta tiles (|w3| <= w3max bounds the second tile too)
-            const float am = block_amax256(d_raw * s_w3max[net], s_w);
+            const float am = block_amax256(fmaxf(fabsf(d_raw[0]), fabsf(d_raw[1])) * s_w3max[net], s_w);
             cs = am > 0.f ? pow2_factor(am) : 1.0f;
-            const float d_o = d_raw * cs;
-            if (half == 0) {
-              float d8[8] = {d_o, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-              tile_put8(o8h, o8l, row, 0, d8);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              d_o[h] = d_raw[h] * cs;
+              if ((tid & 3) == 0) {
+                const float d8[8] = {d_o[h], 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+                tile_put8(o8h, o8l, fr + 8 * h, 0, d8);
+              }
             }
 #pragma unroll
-            for (int qq = 0; qq < 4; ++qq) {
-              const int q = 4 * half + qq;
-              float v[8];
-#pragma unroll
-              for (int i = 0; i < 8; ++i) v[i] = ((m2 >> (qq * 8 + i)) & 1u) ? l4d_ld1(M.att_w3[net] + q * 8 + i) * d_o : 0.f;
-              tile_put8(t3h, t3l, row, q, v);
-            }
+            for (int i = 0; i < 32; ++i)
+              v[i] = ((m2 >> i) & 1u) ? l4d_ld1(M.att_w3[net] + 8 * (i >> 2) + frag_col() + (i & 1)) * d_o[(i >> 1) & 1] : 0.f;
+            frag_put<64>(t3h, t3l, 128, m0, 0, v);
           }
           publish();
           const float inv = 1.0f / cs;
@@ -719,37 +719,25 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
           mma_tt<32>(aT1h, aT1l, aT3h + (uint32_t)wg * 4u * 2048u, aT3l + (uint32_t)wg * 4u * 2048u, [&](int r, int c, float x, float y) {
             red2(G.att_w2t[net] + (size_t)r * 64 + 32 * wg + c, x * inv, y * inv);
           });
-          // dH1[128 x 64] = dH2 * W2
-          mma_prop<64>(S, 0, aT3h, aT3l, 8, sb + L.wa2[net], 64);
-          __syncthreads();
+          // dH1[64 x 64] = dH2 * W2 on this warpgroup's rows
+          mma_prop<64>(d, m0, aT3h, aT3l, 8, sb + L.wa2[net], 64);
           float cs2;
-          {   // re-scale the propagated delta with its own amax, then dH1 * relu1 -> T2 (H2 is dead)
+          {   // re-scale the propagated delta with its own amax, then dH1 * relu1 -> T2 (H2 is dead past the barrier)
             float am = 0.f;
-            float vv[2][16];
 #pragma unroll
-            for (int qq = 0; qq < 2; ++qq) {
-              acc_ld16(S, (2 * half + qq) * 16, vv[qq]);
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                vv[qq][i] = ((m1 >> (qq * 16 + i)) & 1u) ? vv[qq][i] : 0.f;
-                am = fmaxf(am, fabsf(vv[qq][i]));
-              }
+            for (int i = 0; i < 32; ++i) {
+              v[i] = ((m1 >> i) & 1u) ? d[i] : 0.f;
+              am = fmaxf(am, fabsf(v[i]));
             }
             am = block_amax256(am, s_w);
             const float r = am > 0.f ? pow2_factor(am) : 1.0f;
             cs2 = cs * r;
 #pragma unroll
-            for (int qq = 0; qq < 2; ++qq) {
-              const int q = 2 * half + qq;
-#pragma unroll
-              for (int i = 0; i < 16; ++i) vv[qq][i] *= r;
-              tile_put8(t2h, t2l, row, 2 * q, vv[qq]);
-              tile_put8(t2h, t2l, row, 2 * q + 1, vv[qq] + 8);
-            }
+            for (int i = 0; i < 32; ++i) v[i] *= r;
+            frag_put<64>(t2h, t2l, 128, m0, 0, v);
           }
           const float inv2 = 1.0f / cs2;
           L4D_PH(4);
-          L4D_PH(5);
           publish();
           // dW1g[64 x 16] = dH1^T * [geo,1] (warpgroup w: columns [8w, 8w + 8); column 15 is the ones column)
           mma_tt<8>(aT2h, aT2l, aG16h + (uint32_t)wg * 2048u, aG16l + (uint32_t)wg * 2048u, [&](int r, int c, float x, float y) {
@@ -758,28 +746,32 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
             if (ii + 1 < 15) atomicAdd(G.att_w1t[net] + (size_t)(L4D_ENC + ii + 1) * 64 + r, y * inv2);
             else s_csum[net * 64 + r] += y * inv2;
           });
-          // dG[128 x 16] = dH1 * W1g
-          mma_prop<16>(S, 0, aT2h, aT2l, 8, sb + L.wa1[net], 64);
-          __syncthreads();
+          // dG[64 x 16] = dH1 * W1g on this warpgroup's rows
           {
-            float v[16];
-            acc_ld16(S, 0, v);
+            float g[8];
+            mma_prop<16>(g, m0, aT2h, aT2l, 8, sb + L.wa1[net], 64);
 #pragma unroll
-            for (int i = 0; i < 15; ++i) dgeo[i] = fmaf(v[i], inv2, dgeo[i]);
+            for (int i = 0; i < 8; ++i) dgeo[i] = fmaf(g[i], inv2, dgeo[i]);
           }
-          __syncthreads();
           L4D_PH(6);
         }
       }
 
       // ---------------- P3: sigma MLP backward ----------------
-      float d16[16];
-      d16[0] = active ? dsigma * expf(fminf(fmaxf(out[0], -15.f), 15.f)) : 0.f;
+      // dO fragment: column 0 = dsigma * d(sigma)/d(out0) (lanes with frag_col() == 0), columns 1..15 = dG
+      float ds[2], am = 0.f;
+      bool fact[2];
 #pragma unroll
-      for (int i = 0; i < 15; ++i) d16[1 + i] = active ? dgeo[i] : 0.f;
-      float am = 0.f;
+      for (int h = 0; h < 2; ++h) {
+        fact[h] = (uint32_t)t * 128 + (uint32_t)(fr + 8 * h) < n_steps;
+        ds[h] = fact[h] ? s_dsig[fr + 8 * h] * expf(fminf(fmaxf(out[2 * h], -15.f), 15.f)) : 0.f;
+        if ((tid & 3) == 0) am = fmaxf(am, fabsf(ds[h]));
+      }
 #pragma unroll
-      for (int i = 0; i < 16; ++i) am = fmaxf(am, fabsf(d16[i]));
+      for (int i = 0; i < 8; ++i) {
+        dgeo[i] = (fact[(i >> 1) & 1] && 8 * (i >> 2) + frag_col() + (i & 1) < 15) ? dgeo[i] : 0.f;
+        am = fmaxf(am, fabsf(dgeo[i]));
+      }
       const float amax = block_amax256(am, s_w);
       float* dq = A.sv.dfeat + l4d_dfeat_off(A.sv, ray, j);     // this row in the dfeat tile (float4 per 4 features)
       if (amax == 0.f) {           // nothing flows back through this tile
@@ -792,45 +784,34 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
       const float sc = pow2_factor(amax);
       float inv = 1.0f / sc;
 #pragma unroll
-      for (int i = 0; i < 16; ++i) d16[i] *= sc;
-      {
-        float d8[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) d8[i] = half ? d16[8 + i] : d16[i];
-        tile_put8(o16h, o16l, row, half, d8);
+      for (int i = 0; i < 8; ++i) dgeo[i] *= sc;
+      frag_put16_shift<1>(o16h, o16l, m0, dgeo);
+      if ((tid & 3) == 0) {
+        tile_put1(o16h, o16l, fr, 0, ds[0] * sc);
+        tile_put1(o16h, o16l, fr + 8, 0, ds[1] * sc);
       }
       publish();
-      // dHs[128 x 64] = dO * W2   (W2 stored [k/8][16 rows][8])
-      mma_prop<64>(S, 0, aO16h, aO16l, 2, sb + L.w2, 16);
+      float e[32];
+      // dHs[64 x 64] = dO * W2 on this warpgroup's rows  (W2 stored [k/8][16 rows][8])
+      mma_prop<64>(e, m0, aO16h, aO16l, 2, sb + L.w2, 16);
       // dW2s^T[64 x 16] = Hs^T * dO (warpgroup w: columns [8w, 8w + 8))
       mma_tt<8>(aHh, aHl, aO16h + (uint32_t)wg * 2048u, aO16l + (uint32_t)wg * 2048u, [&](int r, int c, float x, float y) {
         atomicAdd(G.sig_w2 + (size_t)(8 * wg + c) * 64 + r, x * inv);
         atomicAdd(G.sig_w2 + (size_t)(8 * wg + c + 1) * 64 + r, y * inv);
       });
-      __syncthreads();
-      {   // re-scale the propagated delta with its own amax, then dHs * relu -> RH (hidden is dead)
-        float am2 = 0.f;
-        float vv[2][16];
+      {   // re-scale the propagated delta with its own amax, then dHs * relu -> RH (hidden is dead past the barrier)
+        float am2 = 0.f, v[32];
 #pragma unroll
-        for (int qq = 0; qq < 2; ++qq) {
-          acc_ld16(S, (2 * half + qq) * 16, vv[qq]);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            vv[qq][i] = ((msk >> (qq * 16 + i)) & 1u) ? vv[qq][i] : 0.f;
-            am2 = fmaxf(am2, fabsf(vv[qq][i]));
-          }
+        for (int i = 0; i < 32; ++i) {
+          v[i] = ((msk >> i) & 1u) ? e[i] : 0.f;
+          am2 = fmaxf(am2, fabsf(v[i]));
         }
         am2 = block_amax256(am2, s_w);
         const float r = am2 > 0.f ? pow2_factor(am2) : 1.0f;
         inv = 1.0f / (sc * r);
 #pragma unroll
-        for (int qq = 0; qq < 2; ++qq) {
-          const int q = 2 * half + qq;
-#pragma unroll
-          for (int i = 0; i < 16; ++i) vv[qq][i] *= r;
-          tile_put8(hh, hl, row, 2 * q, vv[qq]);
-          tile_put8(hh, hl, row, 2 * q + 1, vv[qq] + 8);
-        }
+        for (int i = 0; i < 32; ++i) v[i] *= r;
+        frag_put<64>(hh, hl, 128, m0, 0, v);
       }
       L4D_PH(7);
       // ---------------- P4: input gradients and first-layer weight gradient ----------------
@@ -851,15 +832,40 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
       __syncthreads();
       x_issue_next(ray, t);              // X is free: fetch the next tile behind the input gradients
       L4D_PH(9);
-      // dX[128 x in_pad] = dHs * W1 (W1 stored [k/8][64 rows][8]) -> dfeat, 16 columns at a time straight from the registers
-      for (int n0 = 0; n0 < (int)A.sv.d_quads * 4; n0 += 16) {
-        mma_prop_frag<16>(aHh, aHl, 8, sb + L.w1 + (uint32_t)(n0 / 8) * 64u * 16u, 64, [&](int r, int c, float x, float y) {
-          const uint32_t jr = (uint32_t)t * 128 + (uint32_t)r;
-          const int col = n0 + c;
-          if (jr < n_steps && col < (int)A.sv.d_quads * 4)
-            *reinterpret_cast<float2*>(A.sv.dfeat + l4d_dfeat_off(A.sv, ray, jr) + (size_t)(col >> 2) * 512 + (col & 3)) =
-                make_float2(x * inv, y * inv);
-        });
+      {
+        // dX[64 x in_pad] = dHs * W1 (W1 stored [k/8][64 rows][8]) on this warpgroup's rows -> dfeat, in column blocks of
+        // 64 straight from the registers: blocks 0 and 1 in flight together, then block 2.  Every block is waited for
+        // before any of its registers is read: storing one block while another is in flight makes ptxas serialize
+        // every wgmma of the kernel (C7514).  The last block may read past W1 into the weights that follow it: those
+        // columns are not stored.
+        const int ncols = (int)A.sv.d_quads * 4;
+        auto issue = [&](float (&d)[32], int n0) {
+          mma_prop_issue<64>(d, m0, aHh, aHl, 8, sb + L.w1 + (uint32_t)(n0 / 8) * 64u * 16u, 64);
+        };
+        auto store = [&](const float (&d)[32], int n0) {
+#pragma unroll
+          for (int i = 0; i < 32; i += 2) {
+            const uint32_t jr = (uint32_t)t * 128 + (uint32_t)(fr + 8 * ((i >> 1) & 1));
+            const int col = n0 + 8 * (i >> 2) + frag_col();
+            if (jr < n_steps && col < ncols)
+              *reinterpret_cast<float2*>(A.sv.dfeat + l4d_dfeat_off(A.sv, ray, jr) + (size_t)(col >> 2) * 512 + (col & 3)) =
+                  make_float2(d[i] * inv, d[i + 1] * inv);
+          }
+        };
+        {
+          float d0[32], d1[32];
+          issue(d0, 0);
+          if (ncols > 64) issue(d1, 64);
+          wg_wait<0>();
+          store(d0, 0);
+          if (ncols > 64) store(d1, 64);
+        }
+        if (ncols > 128) {
+          float d[32];
+          issue(d, 128);
+          wg_wait<0>();
+          store(d, 128);
+        }
       }
       __syncthreads();
       L4D_PH(11);
@@ -882,13 +888,12 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
 }
 
 // =============================================================================================
-// flow MLP (16 -> 64 -> 64 -> 6) on tensor cores
+// flow MLP (16 -> 64 -> 64 -> 6) on tensor cores.  One warpgroup per CTA computes both 64-row blocks of a tile.
 // =============================================================================================
 struct FlowTcSmem {
   uint32_t w0, w1, w2;       // weights
   uint32_t fin;              // 16-wide tile hi|lo (2 x 4 KB)
   uint32_t t1, t2;           // 64-wide tiles hi|lo (32 KB each); the forward uses t1 only
-  uint32_t acc;              // fp32 staging tile
   uint32_t do16;             // 16-wide delta tile hi|lo
   uint32_t total_fwd, total;
 };
@@ -899,7 +904,6 @@ __host__ __device__ inline FlowTcSmem flow_tc_smem() {
   L.w0 = take(16 * 64 * 2); L.w1 = take(64 * 64 * 2); L.w2 = take(64 * 16 * 2);
   L.fin = take(2 * 4096);
   L.t1 = take(32 * 1024);
-  L.acc = take(l4dtc::acc_tile_bytes());
   L.total_fwd = o;
   L.t2 = take(32 * 1024);
   L.do16 = take(2 * 4096);
@@ -918,12 +922,13 @@ __device__ __forceinline__ void flow_copy_weights(unsigned char* dsm, const Flow
   cp(L.w2, M.tc_flo_w2, 64 * 16 * 2);
 }
 
-// flow MLP forward for the 128 samples of the CTA.  fin[16] per thread in, flow[8] out (6 used).
-// Optionally returns the relu patterns and leaves relu(layer-2) in tile t1 and (when H1_OUT) relu(layer-1) in tile h1_out.
+// flow MLP forward for the 128 samples of the CTA.  fin[16] per thread (thread == row) in; out: per 64-row block mb the
+// first 8 columns of the output fragment, flow[mb][2h + e] = flow[row 64 mb + frag_row() + 8h][frag_col() + e] (6 used),
+// and the relu patterns of both hidden layers (frag_relu bits per block).  Leaves relu(layer 2) in tile t1 and, when
+// H1_OUT, relu(layer 1) in tile h1.
 template <bool H1_OUT>
-__device__ __forceinline__ void flow_forward_tc(unsigned char* dsm, uint32_t sb, const FlowTcSmem& L, float* S,
-                                                const float (&fin)[16], float (&flow)[8], uint32_t& m1a,
-                                                uint32_t& m1b, uint32_t& m2a, uint32_t& m2b, unsigned char* h1_hi,
+__device__ __forceinline__ void flow_forward_tc(unsigned char* dsm, uint32_t sb, const FlowTcSmem& L, const float (&fin)[16],
+                                                float (&flow)[2][4], uint32_t (&m1)[2], uint32_t (&m2)[2], unsigned char* h1_hi,
                                                 unsigned char* h1_lo, uint32_t a_h1_hi, uint32_t a_h1_lo) {
   const int tid = threadIdx.x;
   unsigned char *fh = dsm + L.fin, *fl = fh + 4096, *t1h = dsm + L.t1, *t1l = t1h + 16384;
@@ -932,47 +937,30 @@ __device__ __forceinline__ void flow_forward_tc(unsigned char* dsm, uint32_t sb,
   tile_put8(fh, fl, tid, 0, fin);
   tile_put8(fh, fl, tid, 1, fin + 8);
   publish();
-  mma_rows<64>(S, 0, sb + L.fin, sb + L.fin + 4096u, sb + L.w0, 64, 2);
-  __syncthreads();
-  m1a = m1b = m2a = m2b = 0u;
 #pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    float v[16];
-    acc_ld16(S, q * 16, v);
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const int k = q * 16 + i;
-      const bool on = v[i] > 0.f;
-      v[i] = on ? v[i] : 0.f;
-      if (k < 32) m1a |= on ? (1u << k) : 0u; else m1b |= on ? (1u << (k - 32)) : 0u;
-    }
-    tile_put8(y1h, y1l, tid, 2 * q, v);
-    tile_put8(y1h, y1l, tid, 2 * q + 1, v + 8);
+  for (int mb = 0; mb < 2; ++mb) {
+    float d[32];
+    mma_rows<64>(d, 64 * mb, sb + L.fin, sb + L.fin + 4096u, sb + L.w0, 64, 2);
+    m1[mb] = frag_relu<64>(d, d);
+    frag_put<64>(y1h, y1l, 128, 64 * mb, 0, d);
   }
   publish();
-  mma_rows<64>(S, 0, a_y1h, a_y1l, sb + L.w1, 64, 8);
-  __syncthreads();
 #pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    float v[16];
-    acc_ld16(S, q * 16, v);
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const int k = q * 16 + i;
-      const bool on = v[i] > 0.f;
-      v[i] = on ? v[i] : 0.f;
-      if (k < 32) m2a |= on ? (1u << k) : 0u; else m2b |= on ? (1u << (k - 32)) : 0u;
-    }
-    tile_put8(t1h, t1l, tid, 2 * q, v);
-    tile_put8(t1h, t1l, tid, 2 * q + 1, v + 8);
+  for (int mb = 0; mb < 2; ++mb) {
+    float d[32];
+    mma_rows<64>(d, 64 * mb, a_y1h, a_y1l, sb + L.w1, 64, 8);
+    m2[mb] = frag_relu<64>(d, d);
+    if (!H1_OUT) __syncthreads();        // layer 2 overwrites its own input rows
+    frag_put<64>(t1h, t1l, 128, 64 * mb, 0, d);
   }
   publish();
-  mma_rows<16>(S, 0, sb + L.t1, sb + L.t1 + 16384u, sb + L.w2, 16, 8);
-  __syncthreads();
-  float o[16];
-  acc_ld16(S, 0, o);
 #pragma unroll
-  for (int k = 0; k < 8; ++k) flow[k] = o[k];
+  for (int mb = 0; mb < 2; ++mb) {
+    float o[8];
+    mma_rows<16>(o, 64 * mb, sb + L.t1, sb + L.t1 + 16384u, sb + L.w2, 16, 8);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) flow[mb][i] = o[i];
+  }
 }
 }  // namespace l4dtc
 
@@ -982,14 +970,13 @@ __device__ __forceinline__ void flow_forward_tc(unsigned char* dsm, uint32_t sb,
 // round trips need block-wide barriers, and barriers around the long, irregular feature gathers stall warps
 // that would otherwise run free (measured: fusing them doubled the forward at L=16).
 // -------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 2) k_fwd_flow_tc(const __grid_constant__ SplitArgs A) {
+__global__ void __launch_bounds__(128, 4) k_fwd_flow_tc(const __grid_constant__ SplitArgs A) {
   using namespace l4dtc;
   extern __shared__ __align__(128) unsigned char dsm[];
   const DevModel& M = A.M;
   const int tid = threadIdx.x;
   const FlowTcSmem L = flow_tc_smem();
   const uint32_t sb = smem_u32(dsm);
-  float* S = reinterpret_cast<float*>(dsm + L.acc);
   flow_copy_weights(dsm, L, M);
   publish();
   const size_t P = A.sv.P;
@@ -1016,13 +1003,17 @@ __global__ void __launch_bounds__(128, 2) k_fwd_flow_tc(const __grid_constant__ 
 #pragma unroll
       for (int k = 0; k < 16; ++k) A.sv.flow_in[(size_t)k * P + p] = fin[k];
     }
-    float flow[8];
-    uint32_t a, b, c, d;
-    flow_forward_tc<false>(dsm, sb, L, S, fin, flow, a, b, c, d, nullptr, nullptr, 0u, 0u);
-    if (active) {
+    float flow[2][4];
+    uint32_t m1[2], m2[2];
+    flow_forward_tc<false>(dsm, sb, L, fin, flow, m1, m2, nullptr, nullptr, 0u, 0u);
 #pragma unroll
-      for (int k = 0; k < 6; ++k) A.sv.flow[(size_t)k * P + p] = flow[k];
-    }
+    for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const size_t q = base + 64 * mb + frag_row() + 8 * (i >> 1);
+        const int k = frag_col() + (i & 1);
+        if (k < 6 && q < P) A.sv.flow[(size_t)k * P + q] = flow[mb][i];
+      }
     __syncthreads();
   }
 }
@@ -1031,7 +1022,7 @@ __global__ void __launch_bounds__(128, 2) k_fwd_flow_tc(const __grid_constant__ 
 // backward 3/4 on tensor cores: flow MLP backprop + weight gradients; dL/d(flow-MLP input) -> flow_in planes
 // Two 64-wide tiles are enough (each delta tile overwrites the activation tile that has just been consumed).
 // -------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) k_bwd_flow_tc(const __grid_constant__ SplitArgs A) {
+__global__ void __launch_bounds__(128, 2) k_bwd_flow_tc(const __grid_constant__ SplitArgs A) {
   using namespace l4dtc;
   extern __shared__ __align__(128) unsigned char dsm[];
   __shared__ float s_w[32];
@@ -1045,11 +1036,9 @@ __global__ void __launch_bounds__(128) k_bwd_flow_tc(const __grid_constant__ Spl
   const uint32_t aFinH = sb + L.fin, aFinL = aFinH + 4096u;
   const uint32_t aT1h = sb + L.t1, aT1l = aT1h + 16384u, aT2h = sb + L.t2, aT2l = aT2h + 16384u;
   const uint32_t aO16h = sb + L.do16, aO16l = aO16h + 4096u;
-  float* S = reinterpret_cast<float*>(dsm + L.acc);
   flow_copy_weights(dsm, L, M);
   publish();
   const size_t P = A.sv.P;
-  const RaySampling rs = l4d_make_sampling(M.near_lidar, M.far_lidar, A.S, A.perturb, A.seed);
   for (size_t base = (size_t)blockIdx.x * 128; base < P; base += (size_t)gridDim.x * 128) {
     const size_t pp = base + tid;
     const bool active = pp < P;
@@ -1071,9 +1060,9 @@ __global__ void __launch_bounds__(128) k_bwd_flow_tc(const __grid_constant__ Spl
       continue;
     }
     // forward recompute: relu(layer 1) -> T2, relu(layer 2) -> T1, relu patterns
-    float flow[8];
-    uint32_t m1a, m1b, m2a, m2b;
-    flow_forward_tc<true>(dsm, sb, L, S, fin, flow, m1a, m1b, m2a, m2b, t2h, t2l, aT2h, aT2l);
+    float flow[2][4];
+    uint32_t m1[2], m2[2];
+    flow_forward_tc<true>(dsm, sb, L, fin, flow, m1, m2, t2h, t2l, aT2h, aT2l);
     const float sc = pow2_factor(am);
     float inv = 1.0f / sc;
 #pragma unroll
@@ -1081,84 +1070,78 @@ __global__ void __launch_bounds__(128) k_bwd_flow_tc(const __grid_constant__ Spl
     tile_put8(o16h, o16l, tid, 0, g);
     tile_put8(o16h, o16l, tid, 1, g + 8);
     publish();
+    float d[2][32];
     // dH2[128 x 64] = dO * W2 (W2 stored [k/8][16 rows][8]) ; dW2^T[64 x 16] = H2^T * dO
-    mma_prop<64>(S, 0, aO16h, aO16l, 2, sb + L.w2, 16);
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb) mma_prop<64>(d[mb], 64 * mb, aO16h, aO16l, 2, sb + L.w2, 16);
     mma_tt<16>(aT1h, aT1l, aO16h, aO16l, [&](int r, int c, float x, float y) {
       if (c < 6) atomicAdd(G.flo_w2 + (size_t)c * 64 + r, x * inv);
       if (c + 1 < 6) atomicAdd(G.flo_w2 + (size_t)(c + 1) * 64 + r, y * inv);
     });
-    __syncthreads();
-    float cs2;
-    {   // dH2 * relu2, re-scaled -> T1 (H2 is dead: dW2^T has been computed)
-      float a2 = 0.f;
+    // dH2 * relu2, re-scaled -> T1 (H2 is dead once every thread is past the barrier in block_amax128)
+    float a2 = 0.f;
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        float v[16];
-        acc_ld16(S, q * 16, v);
+    for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
-        for (int i = 0; i < 16; ++i) if (l4d_bit(m2a, m2b, q * 16 + i)) a2 = fmaxf(a2, fabsf(v[i]));
+      for (int i = 0; i < 32; ++i) {
+        d[mb][i] = ((m2[mb] >> i) & 1u) ? d[mb][i] : 0.f;
+        a2 = fmaxf(a2, fabsf(d[mb][i]));
       }
-      a2 = block_amax128(a2, s_w);
-      const float r = a2 > 0.f ? pow2_factor(a2) : 1.0f;
-      cs2 = sc * r;
+    a2 = block_amax128(a2, s_w);
+    float r = a2 > 0.f ? pow2_factor(a2) : 1.0f;
+    const float cs2 = sc * r;
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        float v[16];
-        acc_ld16(S, q * 16, v);
+    for (int mb = 0; mb < 2; ++mb) {
 #pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] = l4d_bit(m2a, m2b, q * 16 + i) ? v[i] * r : 0.f;
-        tile_put8(t1h, t1l, tid, 2 * q, v);
-        tile_put8(t1h, t1l, tid, 2 * q + 1, v + 8);
-      }
+      for (int i = 0; i < 32; ++i) d[mb][i] *= r;
+      frag_put<64>(t1h, t1l, 128, 64 * mb, 0, d[mb]);
     }
     inv = 1.0f / cs2;
     publish();
     // dH1[128 x 64] = dH2 * W1 ; dW1^T[64 x 64] = H1^T * dH2
-    mma_prop<64>(S, 0, aT1h, aT1l, 8, sb + L.w1, 64);
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb) mma_prop<64>(d[mb], 64 * mb, aT1h, aT1l, 8, sb + L.w1, 64);
     mma_tt<64>(aT2h, aT2l, aT1h, aT1l, [&](int r, int c, float x, float y) {
       red2(G.flo_w1t + (size_t)r * 64 + c, x * inv, y * inv);
     });
-    __syncthreads();
-    float cs3;
-    {   // dH1 * relu1, re-scaled -> T2 (H1 is dead: dW1^T has been computed)
-      float a3 = 0.f;
+    // dH1 * relu1, re-scaled -> T2 (H1 is dead once every thread is past the barrier in block_amax128)
+    float a3 = 0.f;
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        float v[16];
-        acc_ld16(S, q * 16, v);
+    for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
-        for (int i = 0; i < 16; ++i) if (l4d_bit(m1a, m1b, q * 16 + i)) a3 = fmaxf(a3, fabsf(v[i]));
+      for (int i = 0; i < 32; ++i) {
+        d[mb][i] = ((m1[mb] >> i) & 1u) ? d[mb][i] : 0.f;
+        a3 = fmaxf(a3, fabsf(d[mb][i]));
       }
-      a3 = block_amax128(a3, s_w);
-      const float r = a3 > 0.f ? pow2_factor(a3) : 1.0f;
-      cs3 = cs2 * r;
+    a3 = block_amax128(a3, s_w);
+    r = a3 > 0.f ? pow2_factor(a3) : 1.0f;
+    const float cs3 = cs2 * r;
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        float v[16];
-        acc_ld16(S, q * 16, v);
+    for (int mb = 0; mb < 2; ++mb) {
 #pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] = l4d_bit(m1a, m1b, q * 16 + i) ? v[i] * r : 0.f;
-        tile_put8(t2h, t2l, tid, 2 * q, v);
-        tile_put8(t2h, t2l, tid, 2 * q + 1, v + 8);
-      }
+      for (int i = 0; i < 32; ++i) d[mb][i] *= r;
+      frag_put<64>(t2h, t2l, 128, 64 * mb, 0, d[mb]);
     }
     inv = 1.0f / cs3;
     publish();
     // dFin[128 x 16] = dH1 * W0 ; dW0[64 x 16] = dH1^T * Fin
-    mma_prop<16>(S, 0, aT2h, aT2l, 8, sb + L.w0, 64);
+    // dL/d(flow-MLP input) replaces the saved input in place (every thread read its row above); k_bwd_flowgrid turns it
+    // into flow-grid reductions at full occupancy
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb) {
+      float o[8];
+      mma_prop<16>(o, 64 * mb, aT2h, aT2l, 8, sb + L.w0, 64);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const size_t q = base + 64 * mb + frag_row() + 8 * ((i >> 1) & 1);
+        const int k = 8 * (i >> 2) + frag_col() + (i & 1);
+        if (q < P) A.sv.flow_in[(size_t)k * P + q] = o[i] * inv;
+      }
+    }
     mma_tt<16>(aT2h, aT2l, aFinH, aFinL, [&](int r, int c, float x, float y) {
       atomicAdd(G.flo_w0t + (size_t)c * 64 + r, x * inv);
       atomicAdd(G.flo_w0t + (size_t)(c + 1) * 64 + r, y * inv);
     });
-    __syncthreads();
-    float dfin[16];
-    acc_ld16(S, 0, dfin);
-    if (active) {
-      // dL/d(flow-MLP input) replaces the saved input in place (same thread, same addresses); k_bwd_flowgrid
-      // turns it into flow-grid reductions at full occupancy
-#pragma unroll
-      for (int k = 0; k < 16; ++k) A.sv.flow_in[(size_t)k * P + p] = dfin[k] * inv;
-    }
     __syncthreads();
   }
 }

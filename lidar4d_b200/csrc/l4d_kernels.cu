@@ -1139,8 +1139,8 @@ static void fill_split(SplitArgs& A, const L4DConfig* cfg, const void* staged, c
 
 // Dynamic shared memory of the tensor-core kernels: the carve-up plus the 128-byte alignment of its base
 static size_t tc_dyn_smem(uint32_t bytes) { return (size_t)bytes + 128; }
-// the tensor-core dense kernels hold a 128 x sigma_in_pad fp16 hi|lo tile and an fp32 staging tile in shared memory;
-// on sm_90 (227 KB per CTA) the backward's carve-up fits up to 176 inputs (L <= 16)
+// the tensor-core dense kernels hold a 128 x sigma_in_pad fp16 hi|lo tile in shared memory; on sm_90 (227 KB per CTA)
+// the backward's carve-up (196 KB) fits the largest input a valid configuration has (176: 16 hash levels, 4 plane scales)
 static bool use_tc_dense(const L4DConfig* cfg) {
   static int optin = 0;
   if (!optin) {

@@ -7,9 +7,9 @@
 // A thread that owns a row writes one 16-byte chunk per store: conflict-free.
 //
 // MMAs are warpgroup-wide (wgmma.mma_async, m64nNk16, fp32 accumulators in registers).  A 128-row product is two
-// 64-row blocks; in a 256-thread CTA each warpgroup computes one.  Epilogues that work on whole rows (thread == row)
-// read the accumulators from an fp32 staging tile in shared memory (AccTile); weight-gradient products are flushed
-// straight from the registers.
+// 64-row blocks; in a 256-thread CTA each warpgroup computes one.  Epilogues work on the accumulator fragments in the
+// registers: activations go back to operand tiles with frag_put, per-row reductions are quad shuffles, weight-gradient
+// products are flushed straight from the registers.
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -59,10 +59,6 @@ __device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes
 
 // ---- wgmma ---------------------------------------------------------------------------------
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_commit_wait() {
-  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
-  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
-}
 
 // D[64 x N] (+)= A[64 x 16] * B[16 x N]; TA / TB = 1 selects an MN-major operand.  acc == 0 overwrites D.
 template <int N, int TA, int TB>
@@ -107,15 +103,25 @@ struct Opnd {
   uint32_t addr[3];
   uint32_t kstep, lbo, sbo;
 };
-// D[64 x N] = sum over terms t of A_t * B_t over ksteps K=16 steps; warpgroup-wide, returns with D in registers
+// issue D[64 x N] = sum over terms t of A_t * B_t over ksteps K=16 steps as one wgmma group; warpgroup-wide.
+// D must not be touched before a wg_wait that covers the group.
 template <int N, int TA, int TB>
-__device__ __forceinline__ void wg_gemm(float (&d)[N / 2], const Opnd& A, const Opnd& B, int nterms, int ksteps) {
+__device__ __forceinline__ void wg_gemm_issue(float (&d)[N / 2], const Opnd& A, const Opnd& B, int nterms, int ksteps) {
   wg_fence();
   for (int t = 0; t < nterms; ++t)
     for (int k = 0; k < ksteps; ++k)
       wgmma_f16<N, TA, TB>(d, smem_desc(A.addr[t] + (uint32_t)k * A.kstep, A.lbo, A.sbo),
                            smem_desc(B.addr[t] + (uint32_t)k * B.kstep, B.lbo, B.sbo), (t | k) ? 1u : 0u);
-  wg_commit_wait();
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+}
+// wait until at most PENDING of this warpgroup's wgmma groups are still in flight
+template <int PENDING>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
+// D[64 x N] = sum over terms t of A_t * B_t; returns with D in registers
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wg_gemm(float (&d)[N / 2], const Opnd& A, const Opnd& B, int nterms, int ksteps) {
+  wg_gemm_issue<N, TA, TB>(d, A, B, nterms, ksteps);
+  wg_wait<0>();
 }
 // visit the accumulator fragment of a 64 x N product: f(row, col, v[col], v[col + 1]) for the thread's element pairs
 template <int N, class F>
@@ -128,25 +134,37 @@ __device__ __forceinline__ void frag_foreach(const float (&d)[N / 2], F&& f) {
   }
 }
 
-// ---- fp32 accumulator staging tile: 128 rows x 64 columns, float4 groups XOR-swizzled by row ----------
-__host__ __device__ constexpr uint32_t acc_tile_bytes() { return 128u * 64u * 4u; }
-__device__ __forceinline__ int acc_idx(int r, int c) { return r * 64 + ((((c >> 2) ^ r) & 15) << 2) + (c & 3); }
-// fragment of rows [m0, m0 + 64), columns [c0, c0 + N) -> staging tile
+// ---- epilogues in the fragment layout ------------------------------------------------------
+// Thread t of a warpgroup holds rows frag_row() and frag_row() + 8 of the 64-row block and, per 8-column group j,
+// columns 8j + frag_col() + {0, 1}:  d[4j + 2h + e] = D[frag_row() + 8h][8j + frag_col() + e].
+__device__ __forceinline__ int frag_row() { const int t = threadIdx.x & 127; return 16 * (t >> 5) + ((t & 31) >> 2); }
+__device__ __forceinline__ int frag_col() { return 2 * (threadIdx.x & 3); }
+
+// fragment (rows [m0, m0 + 64)) -> fp16 hi|lo operand tile [k/8][rows][8], k-chunks [c0, c0 + N/8); hi = rn(v),
+// lo = rn(v - hi).  One 4-byte store per half2: a warp covers 8 consecutive 16-byte rows of a chunk, conflict-free.
 template <int N>
-__device__ __forceinline__ void acc_store(float* S, const float (&d)[N / 2], int m0, int c0) {
-  frag_foreach<N>(d, [&](int r, int c, float a, float b) {
-    *reinterpret_cast<float2*>(S + acc_idx(m0 + r, c0 + c)) = make_float2(a, b);
-  });
-}
-// this thread's row (threadIdx.x % 128), 16 consecutive columns from c0 (c0 % 4 == 0)
-__device__ __forceinline__ void acc_ld16(const float* S, int c0, float (&v)[16]) {
-  const int r = threadIdx.x & 127;
+__device__ __forceinline__ void frag_put(unsigned char* hi, unsigned char* lo, uint32_t rows, int m0, int c0, const float (&d)[N / 2]) {
+  const int r = m0 + frag_row(), q = threadIdx.x & 3;
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float4 q = *reinterpret_cast<const float4*>(S + acc_idx(r, c0 + 4 * i));
-    v[4 * i] = q.x; v[4 * i + 1] = q.y; v[4 * i + 2] = q.z; v[4 * i + 3] = q.w;
-  }
+  for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float a = d[4 * j + 2 * h], b = d[4 * j + 2 * h + 1];
+      const __half2 x = __floats2half2_rn(a, b);
+      const float2 f = __half22float2(x);
+      const __half2 y = __floats2half2_rn(a - f.x, b - f.y);
+      const size_t off = ((size_t)(c0 + j) * rows + r + 8 * h) * 16 + q * 4;
+      *reinterpret_cast<__half2*>(hi + off) = x;
+      *reinterpret_cast<__half2*>(lo + off) = y;
+    }
 }
+// sum over the four lanes that share a fragment row
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+// barrier over the 128 threads of this thread's warpgroup (named barrier 1 + warpgroup; 0 is __syncthreads)
+__device__ __forceinline__ void wg_bar() { asm volatile("bar.sync %0, 128;" ::"r"(1 + (int)(threadIdx.x >> 7)) : "memory"); }
 
 // pack 8 floats into one 16-byte chunk of fp16 (round to nearest)
 __device__ __forceinline__ uint4 pack8_half(const float* f) {
