@@ -245,6 +245,34 @@ int    l4d_density_forward(const L4DConfig* cfg, const void* staged, const L4DFr
 int    l4d_attribute_forward(const L4DConfig* cfg, const void* staged, const float* d, const float* geo,
                              const unsigned char* mask_or_null, uint32_t n, float* out, void* stream);
 
+/* --- LiDAR4D.density / .attribute on explicit points WITH a backward (the reference's field methods are differentiable;
+ *     a LiDAR_Renderer subclass that samples its own points builds its loss on them).  Gradients reach every parameter the
+ *     reference's autograd graph reaches; none flows to x or d.  Same conventions as the render entry points: caller-owned
+ *     buffers, the caller's stream, L4D_EINVAL / L4D_ESIZE for null or short buffers, n == 0 is a no-op; the backwards
+ *     ACCUMULATE (hash tables straight into `grads`, planes and MLP weights into `grad_work`) and the caller runs
+ *     l4d_unstage_grads afterwards.
+ * l4d_density_forward_ex: l4d_density_forward (sigma / geo / features / flow bit for bit the same) that also writes what the
+ *     backward needs into `saved` (l4d_density_saved_bytes(cfg, n) bytes: the flow-MLP inputs, the sigma-MLP input
+ *     features and the backward's scratch).  saved_or_null = NULL is l4d_density_forward.
+ * l4d_density_backward: upstream g_sigma[n] and / or g_geo[n,15] (NULL = zero) with the saved buffer, frame and x of its
+ *     forward.  Every gradient buffer of `grads` must be set.
+ * l4d_attribute_backward: upstream g_out[n,2] of l4d_attribute_forward with the same d / geo / mask (nothing is saved:
+ *     the heads are recomputed).  Writes g_geo[n,15] when not NULL (zero outside the mask); only the intensity_net and
+ *     raydrop_net buffers of `grads` are used (and must be set). */
+size_t l4d_density_saved_bytes(const L4DConfig* cfg, uint32_t n);
+int    l4d_density_forward_ex(const L4DConfig* cfg, const void* staged, const L4DFrame* frame,
+                              const float* x, uint32_t n, float* sigma, float* geo,
+                              float* features_or_null, float* flow_or_null,
+                              void* saved_or_null, size_t saved_bytes, void* stream);
+int    l4d_density_backward(const L4DConfig* cfg, const void* staged, const L4DFrame* frame,
+                            const float* x, uint32_t n, const void* saved, size_t saved_bytes,
+                            const float* g_sigma_or_null, const float* g_geo_or_null,
+                            const L4DMasterGrads* grads, void* grad_work, size_t grad_work_bytes, void* stream);
+int    l4d_attribute_backward(const L4DConfig* cfg, const void* staged, const float* d, const float* geo,
+                              const unsigned char* mask_or_null, uint32_t n, const float* g_out,
+                              float* g_geo_or_null, const L4DMasterGrads* grads,
+                              void* grad_work, size_t grad_work_bytes, void* stream);
+
 /* --- SURVEY 8(f) "next" row 1: the chamfer / nearest-neighbour op of utils/chamfer3D --------------------------
  * Replaces chamfer_cuda.cpp:17-32 `forward(xyz1,xyz2,dist1,dist2,idx1,idx2)` / `backward(...)` (kernels
  * chamfer3D.cu:11-133,154-174).  xyz1[b,n,3], xyz2[b,m,3] fp32 contiguous; dist1[b,n] = squared distance to the

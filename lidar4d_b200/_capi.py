@@ -146,6 +146,7 @@ EXPORTS = [
     "l4d_render_forward", "l4d_grad_work_bytes", "l4d_render_backward", "l4d_unstage_grads",
     "l4d_flow_forward", "l4d_flow_backward", "l4d_hash_indices", "l4d_density_forward", "l4d_attribute_forward", "l4d_chamfer_work_bytes", "l4d_chamfer_forward", "l4d_chamfer_backward", "l4d_tc_selftest", "l4d_tc_selftest2", "l4d_profile_start", "l4d_profile_stop",
     "l4d_stage_params_ex", "l4d_adam_step", "l4d_launch_count", "l4d_render_backward_ex", "l4d_lidar_rays", "l4d_lidar_loss",
+    "l4d_density_saved_bytes", "l4d_density_forward_ex", "l4d_density_backward", "l4d_attribute_backward",
 ]
 
 
@@ -182,6 +183,15 @@ def declare(lib, prefix: str = "l4d_", host_sim: bool = False):
         f("flow_backward").argtypes = [P(L4DConfig), V, P(L4DFrame), V, U32, V, V, P(L4DMasterGrads), V, SZ, V]
         f("hash_indices").argtypes = [P(L4DConfig), U32, U32, V, U32, V, V, V]
         f("density_forward").argtypes = [P(L4DConfig), V, P(L4DFrame), V, U32, V, V, V, V, V]
+        # explicit-point density / attribute with a backward: saved = l4d_density_saved_bytes(cfg, n) bytes, the
+        # backwards accumulate into `grads` / grad_work like l4d_render_backward (then l4d_unstage_grads)
+        lib.l4d_density_saved_bytes.argtypes = [P(L4DConfig), U32]
+        lib.l4d_density_saved_bytes.restype = SZ
+        lib.l4d_density_forward_ex.argtypes = [P(L4DConfig), V, P(L4DFrame), V, U32, V, V, V, V, V, SZ, V]
+        lib.l4d_density_backward.argtypes = [P(L4DConfig), V, P(L4DFrame), V, U32, V, SZ, V, V, P(L4DMasterGrads), V, SZ, V]
+        lib.l4d_attribute_backward.argtypes = [P(L4DConfig), V, V, V, V, U32, V, V, P(L4DMasterGrads), V, SZ, V]
+        for n in ("l4d_density_forward_ex", "l4d_density_backward", "l4d_attribute_backward"):
+            getattr(lib, n).restype = C.c_int
         lib.l4d_attribute_forward.argtypes = [P(L4DConfig), V, V, V, V, U32, V, V]
         lib.l4d_attribute_forward.restype = C.c_int
         lib.l4d_chamfer_work_bytes.argtypes = [U32, U32, U32]

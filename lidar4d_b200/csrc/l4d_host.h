@@ -247,6 +247,24 @@ static inline SavedLayout saved_layout(const L4DConfig* c, uint32_t n_rays, uint
   L.total = o;
   return L;
 }
+// what l4d_density_forward_ex saves for l4d_density_backward on n explicit points: the Lagrange-contracted flow-MLP
+// inputs [16][n] and the sigma-MLP input features [sigma_in_dim][n] as SoA planes (thread == point: every warp access is
+// one 128 B line), and the per-CTA hidden scratch of k_density_bwd, one [64][L4D_NT] column block per CTA.  The backward
+// runs at most `ctas` CTAs (one per 128-point tile, capped at L4D_BWD_SCRATCH_CTAS), so the buffer stays O(n).
+struct DensitySavedLayout { size_t flow_in, feat, hidden, total; uint32_t ctas; };
+static inline DensitySavedLayout density_saved_layout(const L4DConfig* c, uint32_t n) {
+  DensitySavedLayout L;
+  size_t o = 0;
+  auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
+  const uint32_t tiles = (uint32_t)(((size_t)n + L4D_NT - 1) / L4D_NT);
+  L.ctas = tiles < L4D_BWD_SCRATCH_CTAS ? tiles : L4D_BWD_SCRATCH_CTAS;
+  L.flow_in = take((size_t)n * L4D_FLOW_IN * sizeof(float));
+  L.feat = take((size_t)n * c->sigma_in_dim * sizeof(float));
+  L.hidden = take((size_t)L.ctas * L4D_H * L4D_NT * sizeof(float));
+  L.total = o;
+  return L;
+}
+
 // DevModel::hd_con inside the saved buffer of a launch (level offsets, hence plane sizes, are multiples of 8 entries)
 // mode bit 0: dynamic-hash tables, bit 1: time-plane rows
 static inline void point_contracted(const L4DConfig* c, void* saved, uint32_t n_rays, uint32_t S, DevModel& M, int mode) {

@@ -1042,6 +1042,8 @@ __global__ void __launch_bounds__(NT) k_attribute(const __grid_constant__ Attrib
   A.out[2 * i + 1] = o1;
 }
 
+#include "l4d_points.cuh"
+
 // =============================================================================
 // C-ABI launchers
 // =============================================================================
@@ -1531,6 +1533,119 @@ extern "C" int l4d_attribute_forward(const L4DConfig* cfg, const void* staged, c
   const size_t smem = (size_t)(64 + 81 + 129) * NT * sizeof(float);
   L4D_CUDA(cudaFuncSetAttribute(k_attribute<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   ++g_launches; k_attribute<NT><<<nblk(n, NT), NT, smem, (cudaStream_t)stream>>>(A);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+// ---- LiDAR4D.density / .attribute on explicit points with a backward (l4d_points.cuh) ----------------------------
+extern "C" size_t l4d_density_saved_bytes(const L4DConfig* cfg, uint32_t n) {
+  if (check_config(cfg) != L4D_OK) return 0;
+  return density_saved_layout(cfg, n).total;
+}
+
+extern "C" int l4d_density_forward_ex(const L4DConfig* cfg, const void* staged, const L4DFrame* frame, const float* x,
+                                      uint32_t n, float* sigma, float* geo, float* features, float* flow, void* saved,
+                                      size_t saved_bytes, void* stream) {
+  int rc = check_config(cfg);
+  if (rc != L4D_OK) return rc;
+  if (!staged || !frame || !x || !sigma || !geo) return l4d_fail(L4D_EINVAL, "null pointer");
+  if (!saved) return l4d_density_forward(cfg, staged, frame, x, n, sigma, geo, features, flow, stream);
+  const DensitySavedLayout L = density_saved_layout(cfg, n);
+  if (saved_bytes < L.total) return l4d_fail(L4D_ESIZE, "saved buffer too small");
+  if (n == 0) return L4D_OK;
+  DensityTrainArgs A;
+  memset(&A, 0, sizeof(A));
+  build_model(cfg, staged, A.M);
+  A.F = *frame; A.x = x; A.n = n; A.sigma = sigma; A.geo = geo; A.features = features; A.flow = flow;
+  char* b = reinterpret_cast<char*>(saved);
+  A.flow_in = reinterpret_cast<float*>(b + L.flow_in);
+  A.feat = reinterpret_cast<float*>(b + L.feat);
+  const size_t smem = 64 * L4D_NT * sizeof(float);
+  L4D_CUDA(cudaFuncSetAttribute(k_density_train<L4D_NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  ++g_launches; k_density_train<L4D_NT><<<nblk(n, L4D_NT), L4D_NT, smem, (cudaStream_t)stream>>>(A);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+// every gradient sink the point backwards write must be present: l4d_unstage_grads only clears the grad_work regions it
+// folds into a non-null master, and grad_work has to be all zero again after it
+static int check_point_grads(const L4DConfig* cfg, const L4DMasterGrads* g, bool density) {
+  if (!g->intensity_net && !density) return l4d_fail(L4D_EINVAL, "null intensity_net gradient buffer");
+  if (!g->raydrop_net && !density) return l4d_fail(L4D_EINVAL, "null raydrop_net gradient buffer");
+  if (!density) return L4D_OK;
+  if (!g->hash_static || !g->flow_grid || !g->sigma_net) return l4d_fail(L4D_EINVAL, "null gradient buffer");
+  for (int k = 0; k < 3; ++k)
+    if (!g->flow_mlp[k]) return l4d_fail(L4D_EINVAL, "null flow_mlp gradient buffer");
+  for (uint32_t s = 0; s < cfg->n_plane_scales; ++s)
+    for (int ci = 0; ci < 6; ++ci)
+      if (!g->planes[s][ci]) return l4d_fail(L4D_EINVAL, "null plane gradient buffer");
+  for (int p = 0; p < 3; ++p)
+    for (uint32_t s = 0; s < cfg->time_resolution; ++s)
+      if (!g->hash_dynamic[p][s]) return l4d_fail(L4D_EINVAL, "null hash_dynamic gradient buffer");
+  return L4D_OK;
+}
+
+extern "C" int l4d_density_backward(const L4DConfig* cfg, const void* staged, const L4DFrame* frame, const float* x,
+                                    uint32_t n, const void* saved, size_t saved_bytes, const float* g_sigma,
+                                    const float* g_geo, const L4DMasterGrads* grads, void* grad_work,
+                                    size_t grad_work_bytes, void* stream) {
+  int rc = check_config(cfg);
+  if (rc != L4D_OK) return rc;
+  if (!staged || !frame || !x || !saved || !grads || !grad_work) return l4d_fail(L4D_EINVAL, "null pointer");
+  const DensitySavedLayout L = density_saved_layout(cfg, n);
+  if (saved_bytes < L.total) return l4d_fail(L4D_ESIZE, "saved buffer too small");
+  if (grad_work_bytes < grad_work_layout(cfg).total) return l4d_fail(L4D_ESIZE, "grad_work buffer too small");
+  rc = check_point_grads(cfg, grads, true);
+  if (rc != L4D_OK) return rc;
+  if (n == 0 || (!g_sigma && !g_geo)) return L4D_OK;
+  DensityBwdArgs A;
+  memset(&A, 0, sizeof(A));
+  build_model(cfg, staged, A.M);
+  build_grads(cfg, grads, grad_work, A.G);
+  A.F = *frame; A.x = x; A.n = n; A.g_sigma = g_sigma; A.g_geo = g_geo;
+  const char* b = reinterpret_cast<const char*>(saved);
+  A.flow_in = reinterpret_cast<const float*>(b + L.flow_in);
+  A.feat = reinterpret_cast<const float*>(b + L.feat);
+  A.hidden = const_cast<float*>(reinterpret_cast<const float*>(b + L.hidden));
+  const size_t smem = (64 * L4D_NT + 2 * L4D_NT * L4D_TILE_LD) * sizeof(float);
+  int grid;
+  rc = grid_for(k_density_bwd<L4D_NT>, L4D_NT, smem, L.ctas, grid);
+  if (rc != L4D_OK) return rc;
+  if (grid > (int)L.ctas) grid = (int)L.ctas;          // one hidden-scratch block per CTA
+  ++g_launches; k_density_bwd<L4D_NT><<<grid, L4D_NT, smem, (cudaStream_t)stream>>>(A);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+extern "C" int l4d_attribute_backward(const L4DConfig* cfg, const void* staged, const float* d, const float* geo,
+                                      const unsigned char* mask, uint32_t n, const float* g_out, float* g_geo,
+                                      const L4DMasterGrads* grads, void* grad_work, size_t grad_work_bytes, void* stream) {
+  int rc = check_config(cfg);
+  if (rc != L4D_OK) return rc;
+  if (!staged || !d || !geo || !g_out || !grads || !grad_work) return l4d_fail(L4D_EINVAL, "null pointer");
+  if (grad_work_bytes < grad_work_layout(cfg).total) return l4d_fail(L4D_ESIZE, "grad_work buffer too small");
+  rc = check_point_grads(cfg, grads, false);
+  if (rc != L4D_OK) return rc;
+  if (n == 0) return L4D_OK;
+  AttributeBwdArgs A;
+  memset(&A, 0, sizeof(A));
+  build_model(cfg, staged, A.M);
+  {
+    // only the attribute-head sinks are touched; the other master gradients may be null here
+    GradWorkLayout GL = grad_work_layout(cfg);
+    char* b = reinterpret_cast<char*>(grad_work);
+    for (int k = 0; k < 2; ++k) {
+      A.G.att_w1t[k] = reinterpret_cast<float*>(b + GL.att_w1t[k]);
+      A.G.att_w2t[k] = reinterpret_cast<float*>(b + GL.att_w2t[k]);
+      A.G.att_w3[k] = reinterpret_cast<float*>(b + GL.att_w3[k]);
+    }
+  }
+  A.d = d; A.geo = geo; A.mask = mask; A.n = n; A.g_out = g_out; A.g_geo = g_geo;
+  const size_t smem = (64 * L4D_NT + 2 * L4D_NT * L4D_TILE_LD + L4D_ENC * L4D_NT) * sizeof(float);
+  int grid;
+  rc = grid_for(k_attribute_bwd<L4D_NT>, L4D_NT, smem, (n + L4D_NT - 1) / L4D_NT, grid);
+  if (rc != L4D_OK) return rc;
+  ++g_launches; k_attribute_bwd<L4D_NT><<<grid, L4D_NT, smem, (cudaStream_t)stream>>>(A);
   L4D_CUDA(cudaGetLastError());
   return L4D_OK;
 }

@@ -533,6 +533,130 @@ class _FlowFn(torch.autograd.Function):
         return (None,) * 4 + tuple(views[n] if n in flow_names else None for n in eng.names)
 
 
+_HEAD_NAMES = ("intensity_net.params", "raydrop_net.params")
+
+
+class _DensityFn(torch.autograd.Function):
+    """LiDAR4D.density with a backward (l4d_density_forward_ex / l4d_density_backward).  Parameters are inputs as in
+    _RenderFn, with the same two grad modes; the points get no gradient.  Outputs: sigma, geo_feat and, when asked for,
+    the features and the flow (non-differentiable)."""
+
+    @staticmethod
+    def forward(ctx, eng: _Engine, x, frame, want_feats, *params):
+        lib = eng._lib()
+        n = x.shape[0]
+        dev = x.device
+        sigma = torch.empty(n, device=dev)
+        geo = torch.empty(n, 15, device=dev)
+        feats = torch.empty(n, eng.cfg.sigma_in_dim, device=dev) if want_feats else None
+        flow = torch.empty(n, 6, device=dev) if want_feats else None
+        nsaved = lib.l4d_density_saved_bytes(C.byref(eng.ccfg), n)
+        saved = torch.empty(nsaved, dtype=torch.uint8, device=dev)
+        if n:
+            with torch.cuda.device(dev):
+                rc = lib.l4d_density_forward_ex(C.byref(eng.ccfg), eng.staged.data_ptr(), C.byref(frame), x.data_ptr(), n,
+                                                sigma.data_ptr(), geo.data_ptr(), feats.data_ptr() if want_feats else None,
+                                                flow.data_ptr() if want_feats else None, saved.data_ptr(), nsaved,
+                                                eng.stream())
+            _capi.check(lib, rc, "l4d_density_forward_ex")
+        ctx.eng, ctx.frame, ctx.x, ctx.saved, ctx.nsaved, ctx.stage_gen = eng, frame, x, saved, nsaved, eng.stage_gen
+        ctx.set_materialize_grads(False)        # an unused output passes NULL to the kernel instead of zeros
+        if want_feats:
+            ctx.mark_non_differentiable(feats, flow)
+            return sigma, geo, feats, flow
+        return sigma, geo
+
+    @staticmethod
+    def backward(ctx, g_sigma, g_geo, *rest):
+        eng = ctx.eng
+        lib = eng._lib()
+        if ctx.saved is None:
+            raise RuntimeError("density backward: the saved activations were already consumed by an earlier backward")
+        eng.check_generation(ctx.stage_gen, "density backward")
+        x = ctx.x
+        n = x.shape[0]
+        arena = eng.owner.grad_mode == "arena"
+        tab, views = (eng.attach_grads(), None) if arena else _scratch_grads(eng)
+        if n and (g_sigma is not None or g_geo is not None):
+            g_sigma = None if g_sigma is None else g_sigma.contiguous().float()
+            g_geo = None if g_geo is None else g_geo.contiguous().float()
+            work = eng.work()
+            with torch.cuda.device(x.device):
+                rc = lib.l4d_density_backward(C.byref(eng.ccfg), eng.staged.data_ptr(), C.byref(ctx.frame), x.data_ptr(), n,
+                                              ctx.saved.data_ptr(), ctx.nsaved,
+                                              g_sigma.data_ptr() if g_sigma is not None else None,
+                                              g_geo.data_ptr() if g_geo is not None else None,
+                                              C.byref(tab), work.data_ptr(), work.numel(), eng.stream())
+                _capi.check(lib, rc, "l4d_density_backward")
+                rc = lib.l4d_unstage_grads(C.byref(eng.ccfg), work.data_ptr(), work.numel(), C.byref(tab), eng.stream())
+                _capi.check(lib, rc, "l4d_unstage_grads")
+        ctx.saved = None
+        if arena:
+            return (None,) * (4 + len(eng.names))
+        return (None,) * 4 + tuple(None if k in _HEAD_NAMES else views[k] for k in eng.names)
+
+
+def _head_grads(eng: _Engine):
+    """Zeroed gradient buffers of the two attribute heads and a pointer table holding only them (the attribute backward
+    writes no other sink, and l4d_unstage_grads skips null ones)."""
+    ts = eng.tensors()
+    bufs = {k: torch.zeros_like(ts[k]) for k in _HEAD_NAMES}
+    tab = _capi.L4DMasterGrads()
+    tab.intensity_net = bufs["intensity_net.params"].data_ptr()
+    tab.raydrop_net = bufs["raydrop_net.params"].data_ptr()
+    return tab, bufs
+
+
+class _AttributeFn(torch.autograd.Function):
+    """LiDAR4D.attribute with a backward (l4d_attribute_forward / l4d_attribute_backward).  Differentiable w.r.t.
+    geo_feat and the two head nets (inputs w_int, w_drop); d and the mask get no gradient.  Nothing is saved on the GPU:
+    the backward recomputes the heads from d, geo_feat and the mask."""
+
+    @staticmethod
+    def forward(ctx, eng: _Engine, d, geo, m8, w_int, w_drop):
+        lib = eng._lib()
+        n = d.shape[0]
+        ctx.empty = n == 0 or (m8 is not None and not bool(m8.any()))     # host sync, as lidar4d.py:201
+        if ctx.empty:
+            out = torch.zeros(n, 2, device=d.device)
+        else:
+            out = torch.empty(n, 2, device=d.device)
+            with torch.cuda.device(d.device):
+                rc = lib.l4d_attribute_forward(C.byref(eng.ccfg), eng.staged.data_ptr(), d.data_ptr(), geo.data_ptr(),
+                                               m8.data_ptr() if m8 is not None else None, n, out.data_ptr(), eng.stream())
+            _capi.check(lib, rc, "l4d_attribute_forward")
+        ctx.eng, ctx.stage_gen = eng, eng.stage_gen
+        ctx.save_for_backward(d, geo, m8)
+        return out
+
+    @staticmethod
+    def backward(ctx, g_out):
+        eng = ctx.eng
+        lib = eng._lib()
+        eng.check_generation(ctx.stage_gen, "attribute backward")
+        d, geo, m8 = ctx.saved_tensors
+        need_geo = ctx.needs_input_grad[2]
+        need_w = ctx.needs_input_grad[4] or ctx.needs_input_grad[5]
+        if ctx.empty:
+            return None, None, (torch.zeros_like(geo) if need_geo else None), None, None, None
+        n = d.shape[0]
+        g_out = g_out.contiguous().float()
+        g_geo = torch.empty(n, 15, device=d.device) if need_geo else None
+        arena = eng.owner.grad_mode == "arena"
+        tab, bufs = (eng.attach_grads(), None) if (arena and need_w) else _head_grads(eng)
+        work = eng.work()
+        with torch.cuda.device(d.device):
+            rc = lib.l4d_attribute_backward(C.byref(eng.ccfg), eng.staged.data_ptr(), d.data_ptr(), geo.data_ptr(),
+                                            m8.data_ptr() if m8 is not None else None, n, g_out.data_ptr(),
+                                            g_geo.data_ptr() if g_geo is not None else None, C.byref(tab),
+                                            work.data_ptr(), work.numel(), eng.stream())
+            _capi.check(lib, rc, "l4d_attribute_backward")
+            rc = lib.l4d_unstage_grads(C.byref(eng.ccfg), work.data_ptr(), work.numel(), C.byref(tab), eng.stream())
+            _capi.check(lib, rc, "l4d_unstage_grads")
+        gw = (None, None) if (arena or not need_w) else (bufs["intensity_net.params"], bufs["raydrop_net.params"])
+        return (None, None, g_geo, None) + gw
+
+
 # =============================================================================
 # public modules
 # =============================================================================
@@ -706,9 +830,28 @@ class LiDAR4D(LiDAR_Renderer):
         fl = _FlowFn.apply(eng, x, frame, train, *params)
         return {"forward": fl[:, :3], "backward": fl[:, 3:]}
 
-    # ---- LiDAR4D.density (lidar4d.py:139-188), inference / parity only ---------------------------
-    @torch.no_grad()
+    # ---- LiDAR4D.density (lidar4d.py:139-188) -----------------------------------------------------
     def density(self, x, t=None, return_features: bool = False):
+        """x [N,3] in [-bound, bound] -> {"sigma" [N], "geo_feat" [N,15]} (+ "features", "flow" with return_features).
+        In grad mode, when a parameter requires grad, sigma and geo_feat are differentiable w.r.t. every parameter the
+        reference's density reaches: planes, static hash, the current time's dynamic-hash slices (the warped queries are
+        no_grad there too), flow grid and flow MLP, sigma net.  No gradient flows to x (as render() treats its rays);
+        features and flow are non-differentiable.  Otherwise this is an inference call with no saved state."""
+        if torch.is_grad_enabled() and any(p.requires_grad for p in self._params_list()):
+            eng = self._engine
+            x = x.detach().contiguous().view(-1, 3).float()
+            eng._require_cuda(x)
+            eng.ensure_staged()
+            frame = eng.frame(t)
+            out = _DensityFn.apply(eng, x, frame, bool(return_features), *self._params_list())
+            res = {"sigma": out[0], "geo_feat": out[1]}
+            if return_features:
+                res.update(features=out[2], flow=out[3])
+            return res
+        return self._density_inference(x, t, return_features)
+
+    @torch.no_grad()
+    def _density_inference(self, x, t=None, return_features: bool = False):
         eng = self._engine
         lib = eng._lib()
         x = x.detach().contiguous().view(-1, 3).float()
@@ -731,11 +874,27 @@ class LiDAR4D(LiDAR_Renderer):
             out.update(features=feats, flow=flow)
         return out
 
-    # ---- LiDAR4D.attribute (lidar4d.py:191-223), inference / parity only; render() has the heads fused in ----
-    @torch.no_grad()
+    # ---- LiDAR4D.attribute (lidar4d.py:191-223); render() has the heads fused in -------------------------------------
     def attribute(self, x, d, mask=None, geo_feat=None, **kwargs):
         """x is unused (as in the reference); d [N,3] unit directions, geo_feat [N,15], mask [N] bool or None.
-        Returns [N,2] = (raydrop, intensity); rows outside the mask are zero."""
+        Returns [N,2] = (raydrop, intensity); rows outside the mask are zero.
+        In grad mode the result is differentiable w.r.t. geo_feat and both head nets (whichever require grad); no
+        gradient flows to d.  An empty mask returns zeros and back-propagates zeros without a launch."""
+        heads = [self._engine.tensors()[k] for k in _HEAD_NAMES]
+        if torch.is_grad_enabled() and (geo_feat.requires_grad or any(p.requires_grad for p in heads)):
+            eng = self._engine
+            d = d.detach().contiguous().view(-1, 3).float()
+            n = d.shape[0]
+            geo = geo_feat.contiguous().view(n, 15).float()
+            eng._require_cuda(d, geo)
+            eng.ensure_staged()
+            m8 = None if mask is None else mask.detach().contiguous().view(n).to(torch.uint8)
+            ts = eng.tensors()
+            return _AttributeFn.apply(eng, d, geo, m8, ts[_HEAD_NAMES[0]], ts[_HEAD_NAMES[1]])
+        return self._attribute_inference(x, d, mask, geo_feat, **kwargs)
+
+    @torch.no_grad()
+    def _attribute_inference(self, x, d, mask=None, geo_feat=None, **kwargs):
         eng = self._engine
         lib = eng._lib()
         d = d.detach().contiguous().view(-1, 3).float()
