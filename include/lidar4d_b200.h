@@ -136,7 +136,7 @@ typedef struct L4DRays {
   const float* rays_o;      /* [n_rays,3] */
   const float* rays_d;      /* [n_rays,3] */
   uint32_t     n_rays;
-  uint32_t     n_steps;     /* num_steps (768) */
+  uint32_t     n_steps;     /* num_steps (768), in [2, 8192]: the reference renders nothing at 1 (empty deltas) */
   uint32_t     perturb;     /* z jitter on/off */
   uint32_t     reserved;
   uint64_t     seed;        /* counter-based jitter stream: u = f(seed, ray_offset+ray, sample) */

@@ -198,7 +198,9 @@ __device__ __forceinline__ float block_amax128(float v, float* s_w) {
 __device__ __forceinline__ float pow2_factor(float amax) {
   int e;
   frexpf(amax, &e);
-  return ldexpf(1.0f, 6 - e);
+  // capped at 2^126: a tile whose amax is below 2^-120 (surface-like rays, transmittance ~1e-30 behind the surface)
+  // would otherwise get an infinite scale, and inf * 0 turns the whole tile's gradients into NaN
+  return ldexpf(1.0f, min(6 - e, 126));
 }
 }  // namespace l4dtc
 

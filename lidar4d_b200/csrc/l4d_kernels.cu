@@ -1059,15 +1059,21 @@ static int sm_count() {
   return n;
 }
 
+// n_steps = 1 is refused: the reference's deltas z[1:] - z[:-1] are empty there, so its weights are [N, 0] and depth,
+// image and weight sum are 0 - an artefact of broadcasting an empty tensor, not a render
+static int check_n_steps(uint32_t n_steps) {
+  if (n_steps < 2 || n_steps > L4D_MAX_TILES * L4D_NT) return l4d_fail(L4D_EINVAL, "n_steps out of range [2, 8192]");
+  return L4D_OK;
+}
+
 extern "C" size_t l4d_saved_bytes(const L4DConfig* cfg, uint32_t n_rays, uint32_t n_steps) {
-  if (check_config(cfg) != L4D_OK) return 0;
+  if (check_config(cfg) != L4D_OK || check_n_steps(n_steps) != L4D_OK) return 0;
   return saved_layout(cfg, n_rays, n_steps).total;
 }
 
 static int check_rays(const L4DRays* r) {
   if (!r || !r->rays_o || !r->rays_d) return l4d_fail(L4D_EINVAL, "null rays");
-  if (r->n_steps < 1 || r->n_steps > L4D_MAX_TILES * L4D_NT) return l4d_fail(L4D_EINVAL, "n_steps out of range [1, 8192]");
-  return L4D_OK;
+  return check_n_steps(r->n_steps);
 }
 
 template <typename K>

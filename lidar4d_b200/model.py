@@ -797,6 +797,10 @@ class LiDAR4D(LiDAR_Renderer):
 
     # ---- LiDAR_Renderer.run (renderer.py:44-140) -----------------------------------------------
     def run(self, rays_o, rays_d, time, num_steps=768, perturb=False, ray_offset=0, **kwargs):
+        if not 2 <= int(num_steps) <= 8192:
+            # at num_steps = 1 the reference's deltas z[..., 1:] - z[..., :-1] are empty: its weights come out [N, 0] and
+            # depth / image / weights_sum 0, an artefact of broadcasting an empty tensor rather than a render
+            raise ValueError(f"num_steps must be in [2, 8192], got {num_steps} (the reference renders nothing below 2 samples)")
         eng = self._engine
         prefix = rays_o.shape[:-1]
         ro = rays_o.detach().contiguous().view(-1, 3).float()

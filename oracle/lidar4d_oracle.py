@@ -193,7 +193,9 @@ def sample_lin(n_steps: int) -> np.ndarray:
     """torch.linspace(0,1,S) exactly as the CUDA kernel computes it (the reference renders on the GPU,
     renderer.py:77): step*j below the midpoint, fma(-step, S-1-j, 1) - ONE rounding - above it.  Pinned against the
     real thing: tests/golden/cuda_linspace.npz was dumped from torch.linspace(device="cuda") on a GPU."""
-    step = np.float32(1.0) / np.float32(n_steps - 1) if n_steps > 1 else np.float32(0)
+    if n_steps < 2:                                  # torch.linspace(0, 1, 1) == [0.]
+        return np.zeros(n_steps, np.float32)
+    step = np.float32(1.0) / np.float32(n_steps - 1)
     j = np.arange(n_steps)
     lo = (step * j.astype(np.float32)).astype(np.float32)
     hi = (1.0 - np.float64(step) * (n_steps - 1 - j).astype(np.float64)).astype(np.float32)   # exact product, one rounding

@@ -38,7 +38,9 @@ def test_struct_sizes_match_header_layout():
     assert C.sizeof(_capi.L4DRays) == 48
 
 
-def test_argument_errors_are_codes_not_crashes():
+def test_argument_errors_return_codes():
+    """Bad configurations and null arguments give error codes, and the saved buffer of a launch is sized for the
+    smallest valid one (1 ray, 2 samples: one-sample rays are themselves an argument error)."""
     lib = _capi.load_library()
     cfg = _capi.make_config(FieldConfig())
     assert lib.l4d_staged_bytes(C.byref(cfg)) > 0
@@ -56,7 +58,7 @@ def test_argument_errors_are_codes_not_crashes():
     # the saved buffer of a launch carries the contracted dynamic tables (3 queries x entries x 4 B) and time-plane rows
     c16 = FieldConfig(n_levels_hash=16)
     n_dyn = sum(int(c16.dynamic_grid(p).offset[-1]) for p in range(3))
-    small, big = lib.l4d_saved_bytes(C.byref(_capi.make_config(c16)), 1, 1), 3 * n_dyn * 4
+    small, big = lib.l4d_saved_bytes(C.byref(_capi.make_config(c16)), 1, 2), 3 * n_dyn * 4
     assert small > big + 3 * 3 * 8 * 4 * sum(c16.min_resolution * m for m in c16.plane_scales)
     fr = _capi.make_frame_struct(make_frame(0.3, 51, 8))
     rays = _capi.L4DRays()
@@ -64,6 +66,36 @@ def test_argument_errors_are_codes_not_crashes():
     assert rc == -1 and lib.l4d_last_error()
     rc = lib.l4d_hash_indices(C.byref(cfg), 9, 0, None, 0, None, None, None)
     assert rc == -1
+
+
+@pytest.mark.parametrize("S", [0, 1, 8193])
+def test_sample_count_out_of_range_is_rejected(S):
+    """The reference renders nothing at num_steps = 1 (its deltas z[1:] - z[:-1] are empty, renderer.py:98-104), and the
+    kernels hold at most L4D_MAX_TILES x 128 samples per ray: both ends are argument errors, before any launch, with
+    every other argument valid (the check is the first thing that fails)."""
+    from lidar4d_b200 import LiDAR4D
+    lib = _capi.load_library()
+    cfg = _capi.make_config(FieldConfig())
+    assert lib.l4d_saved_bytes(C.byref(cfg), 16, S) == 0
+    assert b"n_steps out of range [2, 8192]" in lib.l4d_last_error()
+    for ok in (2, 8192):
+        assert lib.l4d_saved_bytes(C.byref(cfg), 16, ok) > 0
+    fr = _capi.make_frame_struct(make_frame(0.3, 51, 8))
+    fake = 256                                    # never dereferenced: the argument check returns first
+    rays = _capi.L4DRays()
+    rays.rays_o = rays.rays_d = fake
+    rays.n_rays, rays.n_steps = 4, S
+    lib.l4d_last_error()
+    rc = lib.l4d_render_forward(C.byref(cfg), fake, C.byref(fr), C.byref(rays), fake, fake, fake, None, None, None, 0, None)
+    assert rc == -1 and b"n_steps out of range" in lib.l4d_last_error()
+    rc = lib.l4d_render_backward(C.byref(cfg), fake, C.byref(fr), C.byref(rays), fake, 1 << 40, fake, fake, None, None,
+                                 C.byref(_capi.L4DMasterGrads()), fake, 1 << 40, None)
+    assert rc == -1 and b"n_steps out of range" in lib.l4d_last_error()
+    m = LiDAR4D(min_resolution=8, base_resolution=16, max_resolution=64, n_levels_hash=2, log2_hashmap_size=8,
+                hash_size_dynamic=(6, 6, 6), flow_base_resolution=4, flow_max_resolution=32, flow_log2_hashmap_size=8)
+    ro = torch.zeros(1, 4, 3)
+    with pytest.raises(ValueError, match="num_steps"):
+        m.render(ro, ro + 1, torch.tensor([[0.1]]), num_steps=S)
 
 
 def test_product_has_no_cpu_path():

