@@ -299,6 +299,28 @@ int    l4d_lidar_rays(const float* pose, float fov_up, float fov, uint32_t H, ui
 int    l4d_lidar_loss(const float* depth, const float* image2, const float* gt3, uint32_t n, float alpha_d, float alpha_r,
                       float alpha_i, float smooth, float* loss, float* g_depth, float* g_image2, void* stream);
 
+/* --- range image <-> point cloud (utils/convert.py) and the point-cloud metric of PointsMeter (utils/metrics.py:229-279) ---
+ * Images are H x W row-major with 1 <= H, W and H*W <= 2^31; otherwise, and for null required pointers, L4D_EINVAL.
+ * l4d_pano_project = lidar_to_pano_with_intensities: points[n, stride] (stride 3, or 4 with the intensity in column 3) ->
+ *   pano[H,W] (nearest distance per pixel, 0 = empty) and, if not NULL, intensities[H,W], with the reference's float32
+ *   arithmetic and its sequential z-buffer (a zero-distance point empties its pixel, keeping its own intensity; ties go to
+ *   the earlier point).  fov_up / fov are in degrees and double, as the reference's Python floats; points at distance
+ *   >= max_depth, or at a NaN distance, are skipped.  n = 0 gives an empty image.
+ *   work = l4d_pano_project_work_bytes(H, W) bytes (L4D_ESIZE when smaller).
+ * l4d_pano_unproject = pano_to_lidar_with_intensities: every pixel with pano != 0 (NaN included) becomes a row
+ *   (dir * pano[, intensity]) of out[H*W, 4] when intensities is given, else out[H*W, 3], in row-major pixel order;
+ *   the number of rows goes to the DEVICE uint32 *count.  work = l4d_pano_unproject_work_bytes(H, W) bytes.
+ * l4d_point_metrics: squared nearest-neighbour distances dist1[n] and dist2[m] (l4d_chamfer_forward), n, m >= 1 ->
+ *   out[5] = {mean(dist1) + mean(dist2), F-score, precision = count(dist1 < thr)/n, recall = count(dist2 < thr)/m, 0};
+ *   the F-score is 0 where 2pr/(p+r) is NaN.  Deterministic: the same inputs give the same bits. */
+size_t l4d_pano_project_work_bytes(uint32_t H, uint32_t W);
+int    l4d_pano_project(const float* points, uint32_t n, uint32_t stride, double fov_up, double fov, uint32_t H, uint32_t W,
+                        float max_depth, float* pano, float* intensities_or_null, void* work, size_t work_bytes, void* stream);
+size_t l4d_pano_unproject_work_bytes(uint32_t H, uint32_t W);
+int    l4d_pano_unproject(const float* pano, const float* intensities_or_null, uint32_t H, uint32_t W, float fov_up, float fov,
+                          float* out, uint32_t* count, void* work, size_t work_bytes, void* stream);
+int    l4d_point_metrics(const float* dist1, uint32_t n, const float* dist2, uint32_t m, float thr, float* out, void* stream);
+
 /* --- profiling aid: while started, CUDA events are recorded on the launch stream around every kernel of
  *     l4d_render_forward / l4d_render_backward.  l4d_profile_stop returns the number of (kernel name, ms)
  *     pairs written (static strings), or a negative error code.  Not thread-safe. --------------------------- */

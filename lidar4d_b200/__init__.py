@@ -8,8 +8,17 @@ if the library or a CUDA device is missing (there is no CPU fallback).
 from .geometry import FieldConfig, make_frame  # noqa: F401
 
 
+_CONVERT = ("lidar_to_pano_with_intensities", "lidar_to_pano", "pano_to_lidar_with_intensities", "pano_to_lidar")
+
+
 def __getattr__(name):
     if name in ("LiDAR4D", "LiDAR_Renderer"):
         from . import model
         return getattr(model, name)
+    if name in _CONVERT:
+        from . import convert
+        return getattr(convert, name)
+    if name in ("point_metrics", "PointsMeter"):
+        from . import metrics
+        return getattr(metrics, name)
     raise AttributeError(name)

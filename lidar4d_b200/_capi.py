@@ -147,6 +147,8 @@ EXPORTS = [
     "l4d_flow_forward", "l4d_flow_backward", "l4d_hash_indices", "l4d_density_forward", "l4d_attribute_forward", "l4d_chamfer_work_bytes", "l4d_chamfer_forward", "l4d_chamfer_backward", "l4d_tc_selftest", "l4d_tc_selftest2", "l4d_profile_start", "l4d_profile_stop",
     "l4d_stage_params_ex", "l4d_adam_step", "l4d_launch_count", "l4d_render_backward_ex", "l4d_lidar_rays", "l4d_lidar_loss",
     "l4d_density_saved_bytes", "l4d_density_forward_ex", "l4d_density_backward", "l4d_attribute_backward",
+    "l4d_pano_project_work_bytes", "l4d_pano_project", "l4d_pano_unproject_work_bytes", "l4d_pano_unproject",
+    "l4d_point_metrics",
 ]
 
 
@@ -213,6 +215,16 @@ def declare(lib, prefix: str = "l4d_", host_sim: bool = False):
         lib.l4d_lidar_rays.restype = C.c_int
         lib.l4d_lidar_loss.argtypes = [V, V, V, U32, C.c_float, C.c_float, C.c_float, C.c_float, V, V, V, V]
         lib.l4d_lidar_loss.restype = C.c_int
+        lib.l4d_pano_project_work_bytes.argtypes = [U32, U32]
+        lib.l4d_pano_project_work_bytes.restype = SZ
+        lib.l4d_pano_project.argtypes = [V, U32, U32, C.c_double, C.c_double, U32, U32, C.c_float, V, V, V, SZ, V]
+        lib.l4d_pano_project.restype = C.c_int
+        lib.l4d_pano_unproject_work_bytes.argtypes = [U32, U32]
+        lib.l4d_pano_unproject_work_bytes.restype = SZ
+        lib.l4d_pano_unproject.argtypes = [V, V, U32, U32, C.c_float, C.c_float, V, V, V, SZ, V]
+        lib.l4d_pano_unproject.restype = C.c_int
+        lib.l4d_point_metrics.argtypes = [V, U32, V, U32, C.c_float, V, V]
+        lib.l4d_point_metrics.restype = C.c_int
         lib.l4d_launch_count.argtypes = []
         lib.l4d_launch_count.restype = C.c_uint64
         lib.l4d_profile_start.argtypes = []
