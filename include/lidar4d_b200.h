@@ -321,6 +321,43 @@ int    l4d_pano_unproject(const float* pano, const float* intensities_or_null, u
                           float* out, uint32_t* count, void* work, size_t work_bytes, void* stream);
 int    l4d_point_metrics(const float* dist1, uint32_t n, const float* dist2, uint32_t m, float thr, float* out, void* stream);
 
+/* --- the flow loss's point-cloud preparation (utils/misc.py point_removal, model/runner.py process_pointcloud) ---------
+ * Points are row-major [n, 3] float64 unless said otherwise, 1 <= n < 2^31 (else L4D_EINVAL, as for null required
+ * pointers).  Compactions keep index order and write their row counts to DEVICE uint32 memory; work buffers of at least
+ * the matching *_work_bytes(n) bytes are the caller's (L4D_ESIZE when smaller).  Every op runs on `stream`.
+ * l4d_range_filter = range_filter: float32 points[n, stride] (stride >= 3, columns beyond z copied) -> the rows with
+ *   dist_min <= |p| <= dist_max, z_lo < z < z_hi and outside the ego box |x| < 2, |y| < 1, |z| < 2, in float32 as NumPy.
+ * l4d_knn_mean_dist: avg[i] = mean of sqrt(d2) over the min(k, n) nearest points of point i (itself included, 1 <= k
+ *   <= 64), d2 = ((dx*dx) + dy*dy) + dz*dz in float64, summed in ascending order.  Exact selection, no work buffer.
+ * l4d_outlier_select: Open3D's statistical outlier rule on those means: mean = sum_{avg>0} avg / n, std =
+ *   sqrt(sum_{avg>0} (avg - mean)^2 / (n - 1)); keep avg > 0 && avg < mean + std_ratio * std -> out[count, 3] and, if
+ *   not NULL, the kept int32 indices.  stats_or_null (device, 3 doubles) receives {threshold, mean, std}.
+ * l4d_plane_scores: counts[h] = #{i : |((a x_i + b y_i) + c z_i) + d| / r < threshold} for the m hypotheses
+ *   hypotheses[h] = (a, b, c, d, r) (device [m, 5] float64), every operation rounded on its own (no FMA).
+ * l4d_plane_mask: mask[i] = 1 where point i is an inlier of (a, b, c, d, r); other bytes are left as they are, so calls
+ *   on a zeroed mask build the union of several hypotheses' inliers.
+ * l4d_ground_split: ground = rows with mask[i] != 0 && z < z_max, rest = all other rows, each in index order with
+ *   optional int32 indices; counts (device, 2 x uint32) = {ground rows, rest rows}.
+ * l4d_pose_transform: out[i] = (pose @ [scale * p_i, 1])[:3] in float64, ((p_r0 X + p_r1 Y) + p_r2 Z) + p_r3, with
+ *   pose a HOST row-major 4x4 float32 matrix. */
+size_t l4d_range_filter_work_bytes(uint32_t n);
+int    l4d_range_filter(const float* points, uint32_t n, uint32_t stride, float dist_min, float dist_max, float z_lo, float z_hi,
+                        float* out, uint32_t* count, void* work, size_t work_bytes, void* stream);
+int    l4d_knn_mean_dist(const double* points, uint32_t n, uint32_t k, double* avg, void* stream);
+size_t l4d_outlier_select_work_bytes(uint32_t n);
+int    l4d_outlier_select(const double* points, uint32_t n, const double* avg, double std_ratio, double* out,
+                          int32_t* index_or_null, uint32_t* count, double* stats_or_null, void* work, size_t work_bytes,
+                          void* stream);
+int    l4d_plane_scores(const double* points, uint32_t n, const double* hypotheses, uint32_t m, double threshold,
+                        uint32_t* counts, void* stream);
+int    l4d_plane_mask(const double* points, uint32_t n, double a, double b, double c, double d, double r, double threshold,
+                      uint8_t* mask, void* stream);
+size_t l4d_ground_split_work_bytes(uint32_t n);
+int    l4d_ground_split(const double* points, uint32_t n, const uint8_t* mask, double z_max, double* ground,
+                        int32_t* ground_index_or_null, double* rest, int32_t* rest_index_or_null, uint32_t* counts,
+                        void* work, size_t work_bytes, void* stream);
+int    l4d_pose_transform(const double* points, uint32_t n, double scale, const float* pose, double* out, void* stream);
+
 /* --- profiling aid: while started, CUDA events are recorded on the launch stream around every kernel of
  *     l4d_render_forward / l4d_render_backward.  l4d_profile_stop returns the number of (kernel name, ms)
  *     pairs written (static strings), or a negative error code.  Not thread-safe. --------------------------- */

@@ -149,6 +149,9 @@ EXPORTS = [
     "l4d_density_saved_bytes", "l4d_density_forward_ex", "l4d_density_backward", "l4d_attribute_backward",
     "l4d_pano_project_work_bytes", "l4d_pano_project", "l4d_pano_unproject_work_bytes", "l4d_pano_unproject",
     "l4d_point_metrics",
+    "l4d_range_filter_work_bytes", "l4d_range_filter", "l4d_knn_mean_dist", "l4d_outlier_select_work_bytes",
+    "l4d_outlier_select", "l4d_plane_scores", "l4d_plane_mask", "l4d_ground_split_work_bytes", "l4d_ground_split",
+    "l4d_pose_transform",
 ]
 
 
@@ -225,6 +228,20 @@ def declare(lib, prefix: str = "l4d_", host_sim: bool = False):
         lib.l4d_pano_unproject.restype = C.c_int
         lib.l4d_point_metrics.argtypes = [V, U32, V, U32, C.c_float, V, V]
         lib.l4d_point_metrics.restype = C.c_int
+        D, F = C.c_double, C.c_float
+        for n in ("range_filter", "outlier_select", "ground_split"):
+            getattr(lib, f"l4d_{n}_work_bytes").argtypes = [U32]
+            getattr(lib, f"l4d_{n}_work_bytes").restype = SZ
+        lib.l4d_range_filter.argtypes = [V, U32, U32, F, F, F, F, V, V, V, SZ, V]
+        lib.l4d_knn_mean_dist.argtypes = [V, U32, U32, V, V]
+        lib.l4d_outlier_select.argtypes = [V, U32, V, D, V, V, V, V, V, SZ, V]
+        lib.l4d_plane_scores.argtypes = [V, U32, V, U32, D, V, V]
+        lib.l4d_plane_mask.argtypes = [V, U32, D, D, D, D, D, D, V, V]
+        lib.l4d_ground_split.argtypes = [V, U32, V, D, V, V, V, V, V, V, SZ, V]
+        lib.l4d_pose_transform.argtypes = [V, U32, D, V, V, V]
+        for n in ("range_filter", "knn_mean_dist", "outlier_select", "plane_scores", "plane_mask", "ground_split",
+                  "pose_transform"):
+            getattr(lib, f"l4d_{n}").restype = C.c_int
         lib.l4d_launch_count.argtypes = []
         lib.l4d_launch_count.restype = C.c_uint64
         lib.l4d_profile_start.argtypes = []

@@ -99,32 +99,19 @@ __global__ void __launch_bounds__(CV_NT) k_pano_project(const ProjectArgs A) {
   }
 }
 
-struct UnprojectArgs {
-  const float* pano;          // [H*W]
-  const float* inten;         // [H*W] or nullptr
-  uint32_t H, W;
-  float fov_up, fov, pi;
-  uint32_t n_tiles;
-  uint32_t* offsets;          // [n_tiles]: kept pixels per tile (PASS 0), then their exclusive prefix sum (PASS 1)
-  float* out;                 // [H*W, 3 | 4]
-  uint32_t* count;            // device scalar
-};
-
-// pano != 0 as NumPy tests it: NaN is kept, +-0 is not
-__device__ __forceinline__ bool cv_kept(float v) { return v != 0.f; }
-
-// PASS 0: kept pixels per tile of CV_TILE pixels; PASS 1 (one CTA): exclusive scan of the tile counts and the total;
-// PASS 2: every tile scatters its kept pixels to its offset in row-major order (an atomic counter would not keep it)
-template <int PASS>
-__global__ void __launch_bounds__(CV_NT) k_pano_unproject(const UnprojectArgs A) {
+// Order-preserving compaction of elements [0, size) in tiles of CV_TILE, shared by k_pano_unproject and the ground-removal
+// kernels (l4d_ground.cuh).  Op supplies `bool keep(size_t q) const` and `void emit(size_t q, uint32_t pos) const`.
+// PASS 0: kept elements per tile; PASS 1 (one CTA): exclusive scan of the tile counts and the total to *count;
+// PASS 2: every tile scatters its kept elements to its offset in element order (an atomic counter would not keep it)
+template <class Op, int PASS>
+__device__ __forceinline__ void cv_compact(const Op& op, size_t size, uint32_t n_tiles, uint32_t* offsets, uint32_t* count) {
   __shared__ uint32_t s_warp[CV_NT / 32];
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-  const size_t hw = (size_t)A.H * A.W;
   if (PASS == 1) {
     uint32_t carry = 0;
-    for (uint32_t t0 = 0; t0 < A.n_tiles; t0 += CV_NT) {
+    for (uint32_t t0 = 0; t0 < n_tiles; t0 += CV_NT) {
       const uint32_t t = t0 + threadIdx.x;
-      const uint32_t v = t < A.n_tiles ? A.offsets[t] : 0u;
+      const uint32_t v = t < n_tiles ? offsets[t] : 0u;
       uint32_t inc = v;
 #pragma unroll
       for (int o = 1; o < 32; o <<= 1) {
@@ -135,24 +122,23 @@ __global__ void __launch_bounds__(CV_NT) k_pano_unproject(const UnprojectArgs A)
       __syncthreads();
       uint32_t before = carry;
       for (uint32_t w = 0; w < warp; ++w) before += s_warp[w];
-      if (t < A.n_tiles) A.offsets[t] = before + inc - v;
+      if (t < n_tiles) offsets[t] = before + inc - v;
       uint32_t total = 0;
       for (int w = 0; w < CV_NT / 32; ++w) total += s_warp[w];
       carry += total;
       __syncthreads();
     }
-    if (threadIdx.x == 0) *A.count = carry;
+    if (threadIdx.x == 0) *count = carry;
     return;
   }
-  const int ostride = A.inten ? 4 : 3;
-  for (uint32_t t = blockIdx.x; t < A.n_tiles; t += gridDim.x) {
+  for (uint32_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
     const size_t base = (size_t)t * CV_TILE;
     if (PASS == 0) {
       uint32_t c = 0;
 #pragma unroll
       for (int j = 0; j < CV_PIX; ++j) {
         const size_t q = base + (size_t)j * CV_NT + threadIdx.x;
-        c += (q < hw && cv_kept(A.pano[q])) ? 1u : 0u;
+        c += (q < size && op.keep(q)) ? 1u : 0u;
       }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
@@ -161,16 +147,15 @@ __global__ void __launch_bounds__(CV_NT) k_pano_unproject(const UnprojectArgs A)
       if (threadIdx.x == 0) {
         uint32_t s = 0;
         for (int w = 0; w < CV_NT / 32; ++w) s += s_warp[w];
-        A.offsets[t] = s;
+        offsets[t] = s;
       }
       __syncthreads();
       continue;
     }
-    uint32_t off = A.offsets[t];
-    for (int j = 0; j < CV_PIX; ++j) {          // row j of the tile = CV_NT consecutive pixels, in pixel order
+    uint32_t off = offsets[t];
+    for (int j = 0; j < CV_PIX; ++j) {          // row j of the tile = CV_NT consecutive elements, in element order
       const size_t q = base + (size_t)j * CV_NT + threadIdx.x;
-      const float v = q < hw ? A.pano[q] : 0.f;
-      const bool keep = q < hw && cv_kept(v);
+      const bool keep = q < size && op.keep(q);
       const uint32_t ballot = __ballot_sync(0xffffffffu, keep);
       if (lane == 0) s_warp[warp] = __popc(ballot);
       __syncthreads();
@@ -180,22 +165,46 @@ __global__ void __launch_bounds__(CV_NT) k_pano_unproject(const UnprojectArgs A)
         if (w < warp) pos += s_warp[w];
         row_total += s_warp[w];
       }
-      if (keep) {
-        // beta = -(i - W/2)/W*2*pi, alpha = (fov_up - j/H*fov)/180*pi: convert.py:112-116 in float32, op by op
-        const float ci = (float)(q % A.W), rj = (float)(q / A.W);
-        const float beta = __fmul_rn(__fmul_rn(__fdiv_rn(-__fsub_rn(ci, (float)A.W * 0.5f), (float)A.W), 2.0f), A.pi);
-        const float alpha = __fmul_rn(__fdiv_rn(__fsub_rn(A.fov_up, __fmul_rn(__fdiv_rn(rj, (float)A.H), A.fov)), 180.0f), A.pi);
-        const float ca = cosf(alpha);
-        float* o = A.out + (size_t)pos * ostride;
-        o[0] = __fmul_rn(__fmul_rn(ca, cosf(beta)), v);
-        o[1] = __fmul_rn(__fmul_rn(ca, sinf(beta)), v);
-        o[2] = __fmul_rn(sinf(alpha), v);
-        if (A.inten) o[3] = A.inten[q];
-      }
+      if (keep) op.emit(q, pos);
       off += row_total;
       __syncthreads();
     }
   }
+}
+
+// pano != 0 as NumPy tests it: NaN is kept, +-0 is not
+__device__ __forceinline__ bool cv_kept(float v) { return v != 0.f; }
+
+struct UnprojectArgs {
+  const float* pano;          // [H*W]
+  const float* inten;         // [H*W] or nullptr
+  uint32_t H, W;
+  float fov_up, fov, pi;
+  uint32_t n_tiles;
+  uint32_t* offsets;          // [n_tiles]: kept pixels per tile (PASS 0), then their exclusive prefix sum (PASS 1)
+  float* out;                 // [H*W, 3 | 4]
+  uint32_t* count;            // device scalar
+
+  __device__ __forceinline__ bool keep(size_t q) const { return cv_kept(pano[q]); }
+  __device__ __forceinline__ void emit(size_t q, uint32_t pos) const {
+    // beta = -(i - W/2)/W*2*pi, alpha = (fov_up - j/H*fov)/180*pi: convert.py:112-116 in float32, op by op
+    const float v = pano[q];
+    const float ci = (float)(q % W), rj = (float)(q / W);
+    const float beta = __fmul_rn(__fmul_rn(__fdiv_rn(-__fsub_rn(ci, (float)W * 0.5f), (float)W), 2.0f), pi);
+    const float alpha = __fmul_rn(__fdiv_rn(__fsub_rn(fov_up, __fmul_rn(__fdiv_rn(rj, (float)H), fov)), 180.0f), pi);
+    const float ca = cosf(alpha);
+    float* o = out + (size_t)pos * (inten ? 4 : 3);
+    o[0] = __fmul_rn(__fmul_rn(ca, cosf(beta)), v);
+    o[1] = __fmul_rn(__fmul_rn(ca, sinf(beta)), v);
+    o[2] = __fmul_rn(sinf(alpha), v);
+    if (inten) o[3] = inten[q];
+  }
+};
+
+// every pixel with pano != 0 becomes a row, in row-major pixel order: cv_compact over the H*W pixels
+template <int PASS>
+__global__ void __launch_bounds__(CV_NT) k_pano_unproject(const UnprojectArgs A) {
+  cv_compact<UnprojectArgs, PASS>(A, (size_t)A.H * A.W, A.n_tiles, A.offsets, A.count);
 }
 
 // PointsMeter.update after the chamfer op, dist1 / dist2 = squared distances: out = {cd, fscore, p1, p2, 0} with

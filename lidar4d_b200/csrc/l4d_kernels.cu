@@ -1686,6 +1686,7 @@ extern "C" int l4d_tc_selftest2(const void* A, const void* B, float* Cout, uint3
 #include "l4d_chamfer.cuh"
 #include "l4d_rays.cuh"
 #include "l4d_convert.cuh"
+#include "l4d_ground.cuh"
 
 #ifdef L4D_PHASE_CLOCKS
 // debug build only: per-phase clock sums of k_bwd_dense_tc (thread 0 of every CTA), cleared on read
