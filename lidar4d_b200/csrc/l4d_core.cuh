@@ -746,8 +746,9 @@ L4D_HD void l4d_agg_weights(const L4DFrame& F, float& wc, float& wf, float& wb) 
   wc = 0.5f + (F.has_fwd ? 0.f : 0.25f) + (F.has_bwd ? 0.f : 0.25f);
 }
 
-// all encoder features of one sample given its flow; order = cat([plane_s, plane_d, hash_s, hash_d])
-template <bool ACC>
+// all encoder features of one sample given its flow; order = cat([plane_s, plane_d, hash_s, hash_d]).
+// STATIC_HASH = false leaves out the static-hash rows: the split pipeline gathers them level-major (l4d_static_sweep, l4d_split.cuh).
+template <bool ACC, bool STATIC_HASH = true>
 L4D_HD void l4d_gather_features(const DevModel& M, const L4DFrame& F, float x, float y, float z, const float (&flow)[8],
                                 float* xb, int xs, const FeatSink& sink, float (&acc)[L4D_H]) {
   const int nS = (int)M.n_scales;
@@ -811,7 +812,7 @@ L4D_HD void l4d_gather_features(const DevModel& M, const L4DFrame& F, float x, f
 
   // ---- static hash (hash_field.py:141-144) ----
 #pragma unroll 1
-  for (int l = 0; l < L; ++l) {
+  for (int l = 0; STATIC_HASH && l < L; ++l) {
     float f[4];
     l4d_encode3_f4(M.gs, M.hs, l, x, y, z, f);
 #pragma unroll

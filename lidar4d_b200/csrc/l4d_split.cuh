@@ -30,18 +30,55 @@ struct SplitArgs {
   SavedView sv;
 };
 
+// static-hash rows of k_fwd_gather, LEVEL-MAJOR (the forward twin of k_bwd_scatter_static).  The fp16 static table is 4 MB per
+// hashed level (64 MB at L = 16, more than the H100's 50 MB L2): gathered sample-major, all levels are live at once.  Here every
+// CTA sweeps its samples once per level PAIR, so the chip reads 8 MB of the table at a time.  row_hash_s is a multiple of 16,
+// so a pair fills one 16-byte chunk of an operand-tile row and a warp stores 512 contiguous bytes per half.  Same per-sample
+// function (l4d_encode3_f4) and sink as the sample-major loop of l4d_gather_features: the same bits.
+template <int NT, bool TILE, int NL>
+__device__ __forceinline__ void l4d_static_sweep(const SplitArgs& A, const RaySampling& rs, int l0, float* xb) {
+  const DevModel& M = A.M;
+  const size_t P = A.sv.P;
+  const int row0 = 2 * (int)M.n_scales * 8 + 4 * l0;
+  for (size_t base = (size_t)blockIdx.x * NT; base < P; base += (size_t)gridDim.x * NT) {
+    const size_t p = base + threadIdx.x;
+    if (p >= P) continue;
+    const uint32_t ray = (uint32_t)(p / A.S), j = (uint32_t)(p % A.S);
+    const float zj = l4d_z(rs, A.ray_offset + ray, j);
+    const float x = l4d_x01(__ldg(A.rays_o + 3 * ray), __ldg(A.rays_d + 3 * ray), zj, M.bound);
+    const float y = l4d_x01(__ldg(A.rays_o + 3 * ray + 1), __ldg(A.rays_d + 3 * ray + 1), zj, M.bound);
+    const float z = l4d_x01(__ldg(A.rays_o + 3 * ray + 2), __ldg(A.rays_d + 3 * ray + 2), zj, M.bound);
+#pragma unroll
+    for (int i = 0; i < NL; ++i) {
+      float f[4];
+      l4d_encode3_f4(M.gs, M.hs, l0 + i, x, y, z, f);
+#pragma unroll
+      for (int c = 0; c < 4; ++c) xb[(4 * i + c) * NT] = f[c];
+    }
+    FeatSink sink;
+    sink.feat = TILE ? nullptr : A.sv.feat; sink.P = P; sink.p = p; sink.dense = nullptr;
+    sink.tile = TILE ? A.sv.feat_tc + l4d_feat_tc_off(A.sv, ray, j) : nullptr; sink.tile_lo = A.sv.x_chunks * 2048u;
+    float dummy[L4D_H];
+    l4d_emit<false>(dummy, M, xb, NT, row0, 4 * NL, sink);
+  }
+}
+
 // -------------------------------------------------------------------------------------------
 // forward 1/2: encoders.  thread == sample; writes features, flow-MLP inputs and flow.
 // -------------------------------------------------------------------------------------------
 // FLOW_GIVEN: the flow was already written by k_fwd_flow_tc; then this kernel has no MLP at all.
 // TILE: features go out as the fp16 hi|lo operand tiles of the tensor-core dense kernels (SavedView::feat_tc);
 // the sample space is then walked in whole 128-row tiles so the rows past the end of a ray get zeros.
-// Occupancy of the MLP-free variant, measured at L=16: round 1 (pair-record gathers, ms per 8192 rays): 3 CTAs/SM 12.8, 4: 11.2,
-// 5: 10.2, 6: 9.9, 7: 10.6, 8: 10.7.  Round 2 (contracted dynamic tables: 4-byte gathers, a tenth of the arithmetic; ms per
-// 16,384 rays): 6: 17.7, 8: 16.4 (64 registers, 168 B of spills), 10: 18.1, 12: 20.7 -> 8.  The variant that also runs the flow
-// MLP keeps 64 accumulators live and stays at 4.
+// Two phases, no barrier between them: planes, dynamic hash, padding rows and ones-padding sample-major, then the static hash
+// level-major (l4d_static_sweep).  The phases write disjoint bytes of the tiles, so CTAs that finish the first phase early
+// start the sweep at once; the grid is persistent and its CTAs get equal shares, so they move through the levels together.
+// Occupancy of the MLP-free variant, measured at L = 16 on an H100 80GB HBM3 at a 400 W power limit (ms per launch of 16,384
+// rays, first phase alone): 6 CTAs/SM 18.3 (80 registers, 60 B of spill stores), 7: 18.9 (72, 112 B), 8: 19.9 (64, 160 B),
+// 10: 22.7 (48, 356 B); the level-major static hash alone, as a kernel of its own: 6.7-6.9 at 53 registers (9 CTAs/SM),
+// 8.2 at 12 CTAs/SM (40 registers), 10.3 at 16 (32); both phases in this kernel: 6: 25.3 (80 registers, 20 B of spill
+// stores), 8: 34.8 (64, 172 B) -> 6.  The variant that also runs the flow MLP keeps 64 accumulators live and stays at 4.
 #ifndef L4D_GATHER_MIN_CTAS
-#define L4D_GATHER_MIN_CTAS 8
+#define L4D_GATHER_MIN_CTAS 6
 #endif
 template <int NT, bool FLOW_GIVEN, bool TILE>
 __global__ void __launch_bounds__(NT, FLOW_GIVEN ? L4D_GATHER_MIN_CTAS : 4) k_fwd_gather(const __grid_constant__ SplitArgs A) {
@@ -83,7 +120,7 @@ __global__ void __launch_bounds__(NT, FLOW_GIVEN ? L4D_GATHER_MIN_CTAS : 4) k_fw
     sink.feat = TILE ? nullptr : A.sv.feat; sink.P = P; sink.p = p; sink.dense = nullptr;
     sink.tile = tile; sink.tile_lo = lo_off;
     float dummy[L4D_H];
-    l4d_gather_features<false>(M, A.F, x, y, z, flow, xb, NT, sink, dummy);
+    l4d_gather_features<false, false>(M, A.F, x, y, z, flow, xb, NT, sink, dummy);      // static hash: below
     if (TILE) {                             // tcnn's ones-padding inside the last stored chunk
       for (uint32_t k = M.sigma_in_dim; k < A.sv.x_chunks * 8u; ++k) {
         unsigned char* q = tile + (size_t)(k >> 3) * 2048 + (size_t)(k & 7u) * 2;
@@ -92,6 +129,10 @@ __global__ void __launch_bounds__(NT, FLOW_GIVEN ? L4D_GATHER_MIN_CTAS : 4) k_fw
       }
     }
   }
+  const int L = (int)M.gs.n_levels;
+#pragma unroll 1
+  for (int l = 0; l + 1 < L; l += 2) l4d_static_sweep<NT, TILE, 2>(A, rs, l, xb);
+  if (L & 1) l4d_static_sweep<NT, TILE, 1>(A, rs, L - 1, xb);
 }
 
 // -------------------------------------------------------------------------------------------
@@ -300,9 +341,8 @@ __global__ void __launch_bounds__(NT) k_bwd_dense(const __grid_constant__ SplitA
 // -------------------------------------------------------------------------------------------
 // backward 2/3: scatter dL/dfeature through the encoders (vector REDs), thread == sample.
 // -------------------------------------------------------------------------------------------
-// Round 1: 3 CTAs/SM = 168 registers, almost no spills; at 4 (128 registers) 220 B of spill traffic per thread competed with the
-// REDs / gathers / shuffles for the LSU pipe (12.8 vs 11.8 ms).  Round 2: with the time planes read and reduced as contracted
-// rows the kernel spills 76 B at 128 registers, and 4 CTAs/SM win: 17.9 vs 19.4 ms (3) and 19.3 ms (5) per 16,384 rays.
+// H100 80GB HBM3 at a 400 W power limit, L = 16, ms per launch of 16,384 rays: 3 CTAs/SM 27.1 (168 registers, 16 B of spill
+// stores), 4: 26.3-26.9 (128, 36 B), 5: 29.4 (96, 224 B) -> 4.
 #ifndef L4D_SCATTER_MIN_CTAS
 #define L4D_SCATTER_MIN_CTAS 4
 #endif
@@ -404,8 +444,13 @@ __global__ void __launch_bounds__(NT) k_bwd_flow(const __grid_constant__ SplitAr
 // Feature (l, 2i+c) of a corner gets basis[i] * w_corner * dFin[2l+c].  The coarse levels (cells wider than
 // the span of a warp of consecutive samples) are summed per run of equal cells with segmented warp scans first.
 // -------------------------------------------------------------------------------------------
+// H100 80GB HBM3 at a 400 W power limit, L = 16, ms per launch of 16,384 rays: bound 4 (64 registers, 8 CTAs/SM resident)
+// 5.03, 8 (62) 5.03, 12 (40, 56 B of spills) 5.09, 16 (32, 88 B) 5.18 -> 4.
+#ifndef L4D_FLOWGRID_MIN_CTAS
+#define L4D_FLOWGRID_MIN_CTAS 4
+#endif
 template <int NT>
-__global__ void __launch_bounds__(NT, 4) k_bwd_flowgrid(const __grid_constant__ SplitArgs A) {
+__global__ void __launch_bounds__(NT, L4D_FLOWGRID_MIN_CTAS) k_bwd_flowgrid(const __grid_constant__ SplitArgs A) {
   const DevModel& M = A.M;
   const size_t P = A.sv.P;
   const RaySampling rs = l4d_make_sampling(M.near_lidar, M.far_lidar, A.S, A.perturb, A.seed);
@@ -472,13 +517,17 @@ __global__ void __launch_bounds__(NT, 4) k_bwd_flowgrid(const __grid_constant__ 
 // -------------------------------------------------------------------------------------------
 // L4D_STATIC_AGG_RES (0 = off): at the coarsest levels consecutive samples of a ray share their cell for 2-4 samples (res 512-1200
 // vs ~215 cells along a ray); their 8 x 4 corner values are summed with a segmented warp scan and only the last lane of a run
-// issues the REDs.  The kernel is bound by the L2 atomic rate (96 % of the measured ceiling), the scans are free:
-// 8.93 -> 7.50 ms per 16,384 rays at L = 16 with the four levels up to res 1200 (profiles/r02_v8_ab_contract.txt).
+// issues the REDs.  H100 80GB HBM3 at a 400 W power limit, L = 16, ms per launch of 16,384 rays: res 1200 at bound 5 (54
+// registers, 9 CTAs/SM resident, no spills) 31.1, at bound 12 (40 registers, 16 B of spills) 33.4, at 16 (32, 56 B) 40.7;
+// aggregation off at bound 12 (40, no spills) 35.2 -> 1200 and 5.
 #ifndef L4D_STATIC_AGG_RES
 #define L4D_STATIC_AGG_RES 1200
 #endif
+#ifndef L4D_STATIC_SCATTER_MIN_CTAS
+#define L4D_STATIC_SCATTER_MIN_CTAS (L4D_STATIC_AGG_RES ? 5 : 8)
+#endif
 template <int NT>
-__global__ void __launch_bounds__(NT, L4D_STATIC_AGG_RES ? 5 : 8) k_bwd_scatter_static(const __grid_constant__ SplitArgs A) {
+__global__ void __launch_bounds__(NT, L4D_STATIC_SCATTER_MIN_CTAS) k_bwd_scatter_static(const __grid_constant__ SplitArgs A) {
   const DevModel& M = A.M;
   const size_t P = A.sv.P;
   const RaySampling rs = l4d_make_sampling(M.near_lidar, M.far_lidar, A.S, A.perturb, A.seed);
