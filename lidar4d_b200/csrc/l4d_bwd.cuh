@@ -348,6 +348,126 @@ L4D_WARP_FN void l4d_static_scatter_warp(float* gbase, const uint32_t (&idx)[8],
     }
   }
 }
+// ---- vertex runs: one gradient update per distinct grid vertex of a warp ------------------------------------------------------
+// Consecutive samples of a ray sit in the same or in neighbouring cells of a level, and neighbouring cells share 4 of their 8
+// corners (2 of 4 in 2D), each lane reaching a shared vertex through a different corner slot.  Slot s of a lane is the vertex
+// cell + bits(s).  Between lanes j < i with every |cell_i - cell_j| <= 1, slot s of lane i is slot s + delta of lane j (per axis;
+// delta = cell_i - cell_j); with any |delta| >= 2 they share nothing.  The lanes that touch one vertex are found per slot
+// from the neighbouring lanes only (head: the previous lane does not touch it; tail: the next one does not), and a segmented
+// Hillis-Steele scan carries, per slot, the partial sum of the vertex's run together with an "open" bit (the run starts further
+// back), routing lane i-d's slots onto lane i's.  It is exact for any cell sequence: a vertex whose lanes are not contiguous
+// simply gets one update per contiguous run.  Keyed on cell coordinates, never on table indices, so two vertices that hash to
+// one entry stay two updates.
+template <int D>
+L4D_WARP_FN constexpr unsigned l4d_slots_with_bit(int a) {      // corner slots whose offset along axis a is 1
+  return D == 3 ? (a == 0 ? 0xAAu : (a == 1 ? 0xCCu : 0xF0u)) : (a == 0 ? 0xAu : 0xCu);
+}
+struct VertexRuns {
+  unsigned open;    // slots whose vertex the previous lane also touches
+  unsigned issue;   // slots this lane reduces: it is active and the next lane does not touch that vertex
+  bool any;         // warp-uniform: some lane shares a vertex with its predecessor (else open = 0 everywhere)
+};
+// cell: this lane's cell at the level; seg: lanes only link to a neighbour with the same seg (the ray); inactive lanes link to
+// nobody and issue nothing.  All 32 lanes must call.
+template <int D>
+L4D_WARP_FN VertexRuns l4d_vertex_runs(const int (&cell)[D], int seg, bool active) {
+  constexpr unsigned ALL = (1u << (1 << D)) - 1u;
+  const unsigned lane = threadIdx.x & 31u;
+  const int key = active ? seg : -1;
+  const int prev_key = __shfl_up_sync(0xffffffffu, key, 1);
+  bool linked = lane > 0u && key >= 0 && prev_key == key;
+  int code = 0;                                    // per axis 2 bits: delta + 1 (delta = cell - previous lane's cell)
+#pragma unroll
+  for (int a = 0; a < D; ++a) {
+    const int dlt = cell[a] - __shfl_up_sync(0xffffffffu, cell[a], 1);
+    linked = linked && dlt >= -1 && dlt <= 1;
+    code |= (dlt + 1) << (2 * a);
+  }
+  // what the next lane sees (its link and its delta per axis) comes back through ballots: shuffles only go upwards here
+  const unsigned links = __ballot_sync(0xffffffffu, linked);
+  const unsigned next_bit = lane < 31u ? (1u << (lane + 1u)) : 0u;
+  unsigned prev_sh = linked ? ALL : 0u, next_sh = (links & next_bit) ? ALL : 0u;
+#pragma unroll
+  for (int a = 0; a < D; ++a) {
+    const unsigned hi = l4d_slots_with_bit<D>(a);
+    const int dp = (code >> (2 * a)) & 3;
+    const unsigned up = __ballot_sync(0xffffffffu, linked && dp == 2), down = __ballot_sync(0xffffffffu, linked && dp == 0);
+    prev_sh &= dp == 2 ? ~hi : (dp == 0 ? hi : ALL);          // moved +1 since the previous lane: its upper corners are our lower
+    next_sh &= (up & next_bit) ? hi : ((down & next_bit) ? ~hi : ALL);
+  }
+  VertexRuns r;
+  r.open = prev_sh;
+  r.issue = active ? (ALL & ~next_sh) : 0u;
+  r.any = links != 0u;
+  return r;
+}
+// v[slot][f]: this lane's contribution to the vertex of each slot.  On return the issuing slots (VertexRuns::issue) hold the sum
+// over the vertex's run of lanes.  Steps only while some slot is still open (at most 5).
+template <int D, int F>
+L4D_WARP_FN void l4d_vertex_sum(float (&v)[1 << D][F], const int (&cell)[D], const VertexRuns& r) {
+  constexpr int K = 1 << D;
+  constexpr unsigned ALL = (1u << K) - 1u;
+  unsigned open = r.open;
+  int low = 0;                                     // the cells' low 2 bits: enough to tell delta in {-1, 0, 1}
+#pragma unroll
+  for (int a = 0; a < D; ++a) low |= (cell[a] & 3) << (K + 2 * a);
+#pragma unroll 1
+  for (int d = 1; d < 32 && __ballot_sync(0xffffffffu, open != 0u) != 0u; d <<= 1) {
+    const int m = __shfl_up_sync(0xffffffffu, (int)open | low, d);
+    // an open slot guarantees that lane i-d touches its vertex: |delta| <= 1, and slot s here is slot s + delta there
+    int dc[D];
+    unsigned po = (unsigned)m & ALL;
+#pragma unroll
+    for (int a = 0; a < D; ++a) {
+      dc[a] = (cell[a] - (m >> (K + 2 * a))) & 3;   // 1: +1, 3: -1, 0: same cell along a
+      const unsigned hi = l4d_slots_with_bit<D>(a);
+      const int sh = 1 << a;
+      po = dc[a] == 1 ? (((po >> sh) & ~hi) | (po & hi)) : (dc[a] == 3 ? (((po << sh) & hi) | (po & ~hi)) : po);
+    }
+    float take[K];
+#pragma unroll
+    for (int s = 0; s < K; ++s) take[s] = ((open >> s) & 1u) ? 1.0f : 0.0f;
+    open &= po;
+#pragma unroll
+    for (int f = 0; f < F; ++f) {
+      float t[K];
+#pragma unroll
+      for (int s = 0; s < K; ++s) t[s] = __shfl_up_sync(0xffffffffu, v[s][f], d);
+#pragma unroll
+      for (int a = 0; a < D; ++a) {          // select network, one stage per axis (no dynamically indexed registers)
+        float u[K];
+#pragma unroll
+        for (int s = 0; s < K; ++s) u[s] = (s >> a) & 1 ? (dc[a] == 3 ? t[s & ~(1 << a)] : t[s]) : (dc[a] == 1 ? t[s | (1 << a)] : t[s]);
+#pragma unroll
+        for (int s = 0; s < K; ++s) t[s] = u[s];
+      }
+      // fma(t, 1, v) rounds like t + v; fma(t, 0, v) = v for every finite t
+#pragma unroll
+      for (int s = 0; s < K; ++s) v[s][f] = fmaf(t[s], take[s], v[s][f]);
+    }
+  }
+}
+// one level of the static hash for a warp of consecutive samples: every distinct vertex of the warp gets one 16-byte reduction.
+// At levels where no lane shares a vertex with its neighbour (the fine ones) this is the plain per-lane scatter after one ballot.
+// All 32 lanes must call; lanes without a sample pass active = false and dd = 0.
+L4D_WARP_FN void l4d_static_vertex_scatter_warp(float* gbase, const uint32_t (&idx)[8], const float (&w)[8], const float4 dd,
+                                         const int (&cell)[3], int seg, bool active) {
+  const VertexRuns r = l4d_vertex_runs<3>(cell, seg, active);
+  if (!r.any) {
+    if (active) {
+#pragma unroll
+      for (int c = 0; c < 8; ++c) l4d_red4(gbase + (size_t)idx[c] * 4, w[c] * dd.x, w[c] * dd.y, w[c] * dd.z, w[c] * dd.w);
+    }
+    return;
+  }
+  float v[8][4];
+#pragma unroll
+  for (int c = 0; c < 8; ++c) { v[c][0] = w[c] * dd.x; v[c][1] = w[c] * dd.y; v[c][2] = w[c] * dd.z; v[c][3] = w[c] * dd.w; }
+  l4d_vertex_sum<3, 4>(v, cell, r);
+#pragma unroll
+  for (int c = 0; c < 8; ++c)
+    if ((r.issue >> c) & 1u) l4d_red4(gbase + (size_t)idx[c] * 4, v[c][0], v[c][1], v[c][2], v[c][3]);
+}
 #endif
 
 // sink of a contracted time-plane row
@@ -405,9 +525,12 @@ struct DynHashCursor {
 };
 // up to n (plane, level) pairs of the dynamic-hash gradient: only the (x,t) query carries gradient
 // (lidar4d.py:160-161,169-170 are no_grad)
-template <class DF>
+// WARP_AGG (device): every lane of the warp calls, inactive ones with active = false; the contracted path then sums each
+// vertex over its run of lanes (l4d_vertex_sum) before it reduces.  seg: the lane's ray.
+template <bool WARP_AGG, class DF>
 L4D_HD void l4d_bw_dynhash_slice(const DevModel& M, const L4DFrame& F, const DevGrads& G, float x, float y, float z, float wc,
-                                 const DF& l4d_dfeat_fn, int row_hash_d, DynHashCursor& cur, int n) {
+                                 const DF& l4d_dfeat_fn, int row_hash_d, DynHashCursor& cur, int n, int seg, bool active) {
+  if (!WARP_AGG && !active) return;
   const int L = (int)M.gs.n_levels;
   const bool quads = (L & 3) == 0;             // rows of a plane start on a multiple of 4: one 16-byte load per 4 levels
 #pragma unroll 1
@@ -427,18 +550,38 @@ L4D_HD void l4d_bw_dynhash_slice(const DevModel& M, const L4DFrame& F, const Dev
       // cx ^ h(cy) or cx + cy * res) and fall into the same aligned quad of entries three times out of four: they go out
       // as one 16-byte RED on that quad, 2.5 instead of 4 L2 atomic operations per level (the backward is bound by them:
       // 1.5 SM-cycles per lane-operation whatever its width, profiles/r02_micro_red.txt).
+      // With WARP_AGG each vertex of the warp is first summed over its run of lanes and reduced once, by the run's last lane.
+      float v[4][1] = {{w[0] * d}, {w[1] * d}, {w[2] * d}, {w[3] * d}};
+      unsigned issue = 0xFu;
+#if defined(__CUDA_ARCH__)
+      if (WARP_AGG) {
+        int cell[2];
+        float fa, fb;
+        uint32_t ua, ub;
+        l4d_pos_fract(M.gd[p].scale[l], ca, ua, fa);
+        l4d_pos_fract(M.gd[p].scale[l], cb, ub, fb);
+        cell[0] = (int)ua; cell[1] = (int)ub;
+        const VertexRuns vr = l4d_vertex_runs<2>(cell, seg, active);
+        if (vr.any) l4d_vertex_sum<2, 1>(v, cell, vr);
+        issue = vr.issue;
+      }
+#endif
       float* cb = gcomb + M.gd[p].offset[l];          // level offsets are multiples of 8 entries: quads stay 16-byte aligned
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         const uint32_t i0 = idx[2 * r], i1 = idx[2 * r + 1];
-        const float a = w[2 * r] * d, b = w[2 * r + 1] * d;
-        const bool same = (i0 >> 2) == (i1 >> 2);
-        const uint32_t s0 = i0 & 3u, s1 = same ? (i1 & 3u) : 4u;
-        l4d_red4(cb + (i0 & ~3u), (s0 == 0u ? a : 0.f) + (s1 == 0u ? b : 0.f), (s0 == 1u ? a : 0.f) + (s1 == 1u ? b : 0.f),
-                 (s0 == 2u ? a : 0.f) + (s1 == 2u ? b : 0.f), (s0 == 3u ? a : 0.f) + (s1 == 3u ? b : 0.f));
-        if (!same) l4d_red1(cb + i1, b);
+        const float a = v[2 * r][0], b = v[2 * r + 1][0];
+        const bool e0 = (issue >> (2 * r)) & 1u, e1 = (issue >> (2 * r + 1)) & 1u;
+        if (e0 && e1 && (i0 >> 2) == (i1 >> 2)) {
+          const uint32_t s0 = i0 & 3u, s1 = i1 & 3u;
+          l4d_red4(cb + (i0 & ~3u), (s0 == 0u ? a : 0.f) + (s1 == 0u ? b : 0.f), (s0 == 1u ? a : 0.f) + (s1 == 1u ? b : 0.f),
+                   (s0 == 2u ? a : 0.f) + (s1 == 2u ? b : 0.f), (s0 == 3u ? a : 0.f) + (s1 == 3u ? b : 0.f));
+        } else {
+          if (e0) l4d_red1(cb + i0, a);
+          if (e1) l4d_red1(cb + i1, b);
+        }
       }
-    } else {
+    } else if (active) {
       const float e0 = d * F.cur.basis[0], e1 = d * F.cur.basis[1], e2 = d * F.cur.basis[2], e3 = d * F.cur.basis[3];
       const size_t off = (size_t)M.gd[p].offset[l] * 4;
       float* glo = G.hd[p][F.cur.slice_lo];
@@ -463,7 +606,7 @@ L4D_HD void l4d_bw_dynhash_slice(const DevModel& M, const L4DFrame& F, const Dev
 
 template <bool WARP_AGG, class DF, bool STATIC_HASH = true, int PARTS = L4D_SC_ALL, bool ROWS = false>
 L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrads& G, float x, float y, float z,
-                             const float* flow, const DF& l4d_dfeat_fn, float (&dflow)[6], bool active);
+                             const float* flow, const DF& l4d_dfeat_fn, float (&dflow)[6], bool active, int seg = 0);
 
 template <bool ROWS = false>
 L4D_HD void l4d_bw_scatter(const DevModel& M, const L4DFrame& F, const DevGrads& G, BwSample& s) {
@@ -476,10 +619,10 @@ L4D_HD void l4d_bw_scatter(const DevModel& M, const L4DFrame& F, const DevGrads&
 
 // ROWS: time planes are sampled from DevModel::pl_con and their gradients go to DevGrads::pl_rows (both must be set)
 // WARP_AGG: every lane of the warp must call (lanes without a sample pass active=false and a
-// provider that returns 0; they take part in the plane aggregation with zero contributions)
+// provider that returns 0; they take part in the plane aggregation with zero contributions); seg: the sample's ray
 template <bool WARP_AGG, class DF, bool STATIC_HASH, int PARTS, bool ROWS>
 L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrads& G, float x, float y, float z,
-                             const float* flow, const DF& l4d_dfeat_fn, float (&dflow)[6], bool active) {
+                             const float* flow, const DF& l4d_dfeat_fn, float (&dflow)[6], bool active, int seg) {
 #pragma unroll
   for (int k = 0; k < 6; ++k) dflow[k] = 0.f;
   const int nS = (int)M.n_scales;
@@ -499,7 +642,7 @@ L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrad
   const int hslots = L4D_SCATTER_INTERLEAVE == 2 ? nS * 12 : nS * 3;
   const int hper = L4D_SCATTER_INTERLEAVE ? (3 * L + hslots - 1) / hslots : 0;
 #define L4D_DYNHASH_SLICE(mode, n) \
-  do { if (L4D_SCATTER_INTERLEAVE == (mode) && active) l4d_bw_dynhash_slice(M, F, G, x, y, z, wc, l4d_dfeat_fn, row_hash_d, hc, (n)); } while (0)
+  do { if (L4D_SCATTER_INTERLEAVE == (mode)) l4d_bw_dynhash_slice<WARP_AGG>(M, F, G, x, y, z, wc, l4d_dfeat_fn, row_hash_d, hc, (n), seg, active); } while (0)
 
 #pragma unroll 1
   for (int sc = 0; sc < nS; ++sc) {
@@ -571,11 +714,10 @@ L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrad
     }
   }
 
-  if (!active) return;
   // static hash: dL/dtable[entry] += w_corner * dfeat[0..4)   (the split pipeline does this level-major in
   // k_bwd_scatter_static so that only one level's 8 MB of gradients is live in L2 at a time)
 #pragma unroll 1
-  for (int l = 0; STATIC_HASH && l < L; ++l) {
+  for (int l = 0; STATIC_HASH && active && l < L; ++l) {
     uint32_t idx[8]; float w[8];
     l4d_corners3(M.gs, l, x, y, z, idx, w);
     float dd[4];
@@ -587,7 +729,7 @@ L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrad
   }
 
   // dynamic hash: whatever the slices above did not cover (all of it when L4D_SCATTER_INTERLEAVE == 0)
-  l4d_bw_dynhash_slice(M, F, G, x, y, z, wc, l4d_dfeat_fn, row_hash_d, hc, 3 * L);
+  l4d_bw_dynhash_slice<WARP_AGG>(M, F, G, x, y, z, wc, l4d_dfeat_fn, row_hash_d, hc, 3 * L, seg, active);
 #undef L4D_DYNHASH_SLICE
 }
 

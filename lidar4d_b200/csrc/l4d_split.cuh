@@ -342,7 +342,10 @@ __global__ void __launch_bounds__(NT) k_bwd_dense(const __grid_constant__ SplitA
 // backward 2/3: scatter dL/dfeature through the encoders (vector REDs), thread == sample.
 // -------------------------------------------------------------------------------------------
 // H100 80GB HBM3 at a 400 W power limit, L = 16, ms per launch of 16,384 rays: 3 CTAs/SM 27.1 (168 registers, 16 B of spill
-// stores), 4: 26.3-26.9 (128, 36 B), 5: 29.4 (96, 224 B) -> 4.
+// stores), 4: 26.3-26.9 (128, 36 B), 5: 29.4 (96, 224 B) -> 4 (short runs, before the dynamic hash's vertex runs).  With the
+// contracted time rows (the benchmark's kernel) at 4: 36.1-36.2 ms (128 registers, 36 B of spill stores) before the vertex
+// runs, 31.8-31.9 (128, 48 B) with them; 18.7 with the dynamic hash left out (a scratch build), so the dynamic hash went from
+// 17.5 to about 13.2 ms of it.
 #ifndef L4D_SCATTER_MIN_CTAS
 #define L4D_SCATTER_MIN_CTAS 4
 #endif
@@ -384,7 +387,7 @@ __global__ void __launch_bounds__(NT, MIN_CTAS) k_bwd_scatter(const __grid_const
 #pragma unroll
     for (int k = 0; k < 6; ++k) flow[k] = (PARTS & L4D_SC_TIME_PLANES) ? A.sv.flow[(size_t)k * P + p] : 0.f;
     DfeatFromTile df{A.sv.dfeat + l4d_dfeat_off(A.sv, ray, j), active};
-    l4d_bw_scatter_t<true, DfeatFromTile, false, PARTS, ROWS>(M, A.F, A.G, x, y, z, flow, df, dflow, active);
+    l4d_bw_scatter_t<true, DfeatFromTile, false, PARTS, ROWS>(M, A.F, A.G, x, y, z, flow, df, dflow, active, (int)ray);
     if (active && (PARTS & L4D_SC_TIME_PLANES)) {
 #pragma unroll
       for (int k = 0; k < 6; ++k) A.sv.dflow[(size_t)k * P + p] = dflow[k];
@@ -515,16 +518,25 @@ __global__ void __launch_bounds__(NT, L4D_FLOWGRID_MIN_CTAS) k_bwd_flowgrid(cons
 // Here every CTA sweeps the samples once per level, so the whole
 // chip works on one level at a time and its gradient slab stays L2-resident.
 // -------------------------------------------------------------------------------------------
-// L4D_STATIC_AGG_RES (0 = off): at the coarsest levels consecutive samples of a ray share their cell for 2-4 samples (res 512-1200
-// vs ~215 cells along a ray); their 8 x 4 corner values are summed with a segmented warp scan and only the last lane of a run
-// issues the REDs.  H100 80GB HBM3 at a 400 W power limit, L = 16, ms per launch of 16,384 rays: res 1200 at bound 5 (54
-// registers, 9 CTAs/SM resident, no spills) 31.1, at bound 12 (40 registers, 16 B of spills) 33.4, at 16 (32, 56 B) 40.7;
-// aggregation off at bound 12 (40, no spills) 35.2 -> 1200 and 5.
+// The kernel's time follows the reductions it issues (H100: 31.1 ms at 112.6 RED.128 per sample, 35.2 ms at 128).
+// L4D_STATIC_VERTEX_RUNS (default 1): every level goes through l4d_static_vertex_scatter_warp: at the coarse levels (0-7 at
+// L = 16) consecutive samples share cells or corners, and each distinct vertex of a warp gets one RED (97.4 per sample on the
+// benchmark's rays, scripts/red_count.py); at the fine levels one ballot finds no shared vertex and the lanes issue their 8
+// corners.  0 selects the former path, kept as the A/B reference while the step-time effect under a power cap is open (DESIGN.md
+// 9, item 4): runs of equal cells (l4d_static_scatter_warp) at the levels up to res L4D_STATIC_AGG_RES (113.4 REDs per sample;
+// bench.py::red_counts models this path), per-lane REDs above.
+// H100 80GB HBM3 at a 400 W power limit, L = 16, ms per launch of 16,384 rays: former path at res 1200 and bound 5 (54
+// registers, 9 CTAs/SM resident, no spills) 31.1-31.7, at bound 12 (40 registers, 16 B of spills) 33.4, at 16 (32, 56 B) 40.7,
+// aggregation off at bound 12 (40, no spills) 35.2; vertex runs at bound 4 (96 registers, no spills) 27.4, 5 (94, no spills)
+// 27.1-27.5, 6 (80, 60 B of spill stores) 31.2, 8 (64, 136 B) not run -> 5 either way.
+#ifndef L4D_STATIC_VERTEX_RUNS
+#define L4D_STATIC_VERTEX_RUNS 1
+#endif
 #ifndef L4D_STATIC_AGG_RES
 #define L4D_STATIC_AGG_RES 1200
 #endif
 #ifndef L4D_STATIC_SCATTER_MIN_CTAS
-#define L4D_STATIC_SCATTER_MIN_CTAS (L4D_STATIC_AGG_RES ? 5 : 8)
+#define L4D_STATIC_SCATTER_MIN_CTAS (L4D_STATIC_VERTEX_RUNS || L4D_STATIC_AGG_RES ? 5 : 8)
 #endif
 template <int NT>
 __global__ void __launch_bounds__(NT, L4D_STATIC_SCATTER_MIN_CTAS) k_bwd_scatter_static(const __grid_constant__ SplitArgs A) {
@@ -537,9 +549,8 @@ __global__ void __launch_bounds__(NT, L4D_STATIC_SCATTER_MIN_CTAS) k_bwd_scatter
   for (int l = 0; l < L; ++l) {
     float* gbase = A.G.hs + (size_t)M.gs.offset[l] * 4;
     const size_t dk = l4d_dfeat_k(row_hash_s + 4 * l);     // row_hash_s is a multiple of 16: one float4 per level
-    const bool agg = L4D_STATIC_AGG_RES && M.gs.res[l] <= (uint32_t)L4D_STATIC_AGG_RES;      // warp-uniform
     for (size_t base = (size_t)blockIdx.x * NT; base < P; base += (size_t)gridDim.x * NT) {
-      // whole warps stay together (the aggregated levels shuffle); lanes past the end shadow the last sample with zero gradient
+      // whole warps stay together (the warp sinks shuffle); lanes past the end shadow the last sample with zero gradient
       const size_t pp = base + threadIdx.x;
       const bool active = pp < P;
       const size_t p = active ? pp : P - 1;
@@ -552,20 +563,21 @@ __global__ void __launch_bounds__(NT, L4D_STATIC_SCATTER_MIN_CTAS) k_bwd_scatter
       const float z = l4d_x01(__ldg(A.rays_o + 3 * ray + 2), __ldg(A.rays_d + 3 * ray + 2), zj, M.bound);
       uint32_t idx[8]; float w[8];
       l4d_corners3(M.gs, l, x, y, z, idx, w);
-#if L4D_STATIC_AGG_RES
-      if (agg) {
-        uint32_t cx, cy, cz; float fx, fy, fz;
-        const float sc = M.gs.scale[l];
-        l4d_pos_fract(sc, x, cx, fx); l4d_pos_fract(sc, y, cy, fy); l4d_pos_fract(sc, z, cz, fz);
+      uint32_t cx, cy, cz; float fx, fy, fz;
+      const float sc = M.gs.scale[l];
+      l4d_pos_fract(sc, x, cx, fx); l4d_pos_fract(sc, y, cy, fy); l4d_pos_fract(sc, z, cz, fz);
+#if L4D_STATIC_VERTEX_RUNS
+      const int cell[3] = {(int)cx, (int)cy, (int)cz};
+      l4d_static_vertex_scatter_warp(gbase, idx, w, dd, cell, (int)ray, active);
+#else
+      if (L4D_STATIC_AGG_RES && M.gs.res[l] <= (uint32_t)L4D_STATIC_AGG_RES) {       // warp-uniform
         // equal keys <=> equal cells for neighbouring lanes (their linear cell indices differ by far less than 2^32)
         l4d_static_scatter_warp(gbase, idx, w, dd, (int)(cx + M.gs.res[l] * (cy + M.gs.res[l] * cz)));
-        continue;
-      }
-#endif
-      if (active) {
+      } else if (active) {
 #pragma unroll
         for (int c = 0; c < 8; ++c) l4d_red4(gbase + (size_t)idx[c] * 4, w[c] * dd.x, w[c] * dd.y, w[c] * dd.z, w[c] * dd.w);
       }
+#endif
     }
   }
 }
