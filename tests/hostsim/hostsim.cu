@@ -448,6 +448,17 @@ extern "C" int hs_hash_indices(const L4DConfig* cfg, uint32_t grid_id, uint32_t 
   return L4D_OK;
 }
 
+// l4d_bilerp of n coordinate pairs: idx [n][4] = x0 x1 y0 y1, w [n][6] = wx0 wx1 wy0 wy1 gx_mult gy_mult
+extern "C" int hs_bilerp(const float* cx, const float* cy, uint32_t n, int W, int H, int* idx, float* w) {
+  for (uint32_t i = 0; i < n; ++i) {
+    const Bilerp b = l4d_bilerp(cx[i], W, cy[i], H);
+    idx[4 * i] = b.x0; idx[4 * i + 1] = b.x1; idx[4 * i + 2] = b.y0; idx[4 * i + 3] = b.y1;
+    w[6 * i] = b.wx0; w[6 * i + 1] = b.wx1; w[6 * i + 2] = b.wy0; w[6 * i + 3] = b.wy1;
+    w[6 * i + 4] = b.gx_mult; w[6 * i + 5] = b.gy_mult;
+  }
+  return L4D_OK;
+}
+
 extern "C" int hs_density_forward(const L4DConfig* cfg, const void* staged, const L4DFrame* frame, const float* x, uint32_t n,
                                   float* sigma, float* geo, float* features, float* flow) {
   DevModel M;
