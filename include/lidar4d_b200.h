@@ -162,11 +162,14 @@ int    l4d_stage_params_ex(const L4DConfig* cfg, const L4DMasterParams* master,
                            void* staged, size_t staged_bytes, uint32_t what, void* stream);
 
 /* --- optimiser step (SURVEY.md 8(f) #4; replaces torch.optim.Adam of main_lidar4d.py:298-300 + the re-staging pass) -----
- * Adam (no weight decay, no amsgrad; torch's fused-kernel operation order) over FLAT fp32 arenas: params, grads and the
- * two moment buffers hold every tensor of the hot path at the same offsets (each tensor starts on a multiple of
- * L4D_ADAM_CHUNK floats).  `groups` = sorted, disjoint [begin,end) float ranges with their learning rate (the
- * reference's param groups, lidar4d.py:226-237); ranges not covered are left alone.  grads are multiplied by inv_scale
- * (1/loss-scale) on the fly; zero_grad=1 clears them in the same pass.  If `master` is given (pointers INTO `params`),
+ * Adam (no weight decay, no amsgrad) over FLAT fp32 arenas: params, grads and the two moment buffers hold every tensor
+ * of the hot path at the same offsets (each tensor starts on a multiple of L4D_ADAM_CHUNK floats).  params, exp_avg and
+ * exp_avg_sq come out bit-identical to torch 2.11's fused Adam (torch._fused_adam_ with state_steps = step), including
+ * its fp32 bias corrections, for every input.  `groups` = sorted, disjoint [begin,end) float ranges with their learning
+ * rate (the reference's param groups, lidar4d.py:226-237); ranges not covered are left alone.  grads are MULTIPLIED by
+ * inv_scale (1/loss-scale) on the fly, which equals torch's division by grad_scale exactly when the scale is a power of
+ * two (all GradScaler produces); grads are not written back unscaled.  zero_grad=1 clears the covered ranges of grads in
+ * the same pass.  If `master` is given (pointers INTO `params`),
  * a group that is exactly one hash table also emits that table's fp16 working copy into `staged` (static / flow: cast;
  * dynamic slice t: the lo half of pair t and the hi half of pair t-1), i.e. l4d_stage_params_ex(L4D_STAGE_TABLES) for free. */
 #define L4D_ADAM_CHUNK 1024

@@ -398,8 +398,7 @@ extern "C" int l4d_adam_step(const L4DConfig* cfg, float* params, float* grads, 
   A.p = params; A.g = grads; A.g_rw = grads; A.m = exp_avg; A.v = exp_avg_sq;
   A.n_chunks = n_floats / L4D_ADAM_CHUNK;
   A.beta1 = beta1; A.beta2 = beta2; A.eps = eps; A.inv_scale = inv_scale; A.zero_grad = zero_grad;
-  A.bc1 = (float)(1.0 - pow((double)beta1, (double)step));
-  A.bc2_sqrt = (float)sqrt(1.0 - pow((double)beta2, (double)step));
+  A.step = (float)step;                 // bias corrections: in fp32 on the device, as torch's fused Adam computes them
   A.n_seg = (int)n_groups;
   StagedLayout L;
   char* sb = reinterpret_cast<char*>(staged);

@@ -9,6 +9,7 @@
 //     (they were ~55 and ~35 separate launches: ~0.4 ms of pure launch latency at the reference's 1,024-ray step).
 #pragma once
 #include <cuda_fp16.h>
+#include <math.h>
 #include <stdint.h>
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -29,14 +30,47 @@ struct AdamArgs {
   float* m;
   float* v;
   unsigned long long n_chunks;
-  float beta1, beta2, eps, bc1, bc2_sqrt, inv_scale;
+  float beta1, beta2, eps, step, inv_scale;   // step as a float, like torch's state_steps
   int n_seg;
   uint32_t zero_grad;                  // 1: clear the gradient arena in the same pass (saves the next step's memset)
   float* g_rw;
   AdamSeg seg[L4D_ADAM_MAX_SEGMENTS];
 };
 
+// One element of Adam (no weight decay, no amsgrad, not maximising) in the operation order of torch 2.11's fused Adam,
+// ATen/native/cuda/fused_adam_utils.cuh adam_math, with its fused multiply-adds written out so that contraction cannot
+// change a bit.  step_size = lr / bc1 and bc2_sqrt = sqrtf(bc2), with bc = 1 - powf(beta, (float)step) in fp32 as torch
+// computes them.  The gradient is MULTIPLIED by inv_scale; for a power-of-two loss scale (all GradScaler produces) that
+// is exactly torch's g / grad_scale.  Compiles for the host too (tests/hostsim/adamsim.cu).
+//
+// IEEE sqrtf and division take a slow path on subnormal operands or quotients, and the second moments of rarely touched
+// entries are subnormal (g ~ 1e-20 => g^2 ~ 1e-40).  Both are evaluated on operands scaled by powers of two, but only
+// where the scaled result is provably the unscaled one, so the result equals the plain IEEE formula for EVERY input:
+//   sqrtf(v) = sqrtf(v * 2^64) * 2^-32 for v < 2^64 (the root of a subnormal is normal; v >= 2^64 is left unscaled);
+//   a / den = ((a * 2^64) / den) * 2^-64 when that scaled quotient is 0 or a finite normal >= 2^-62: then a * 2^64 did not
+//   overflow and a / den is normal too (or rounds to 0), so scaling commutes with rounding.  Otherwise (a subnormal or
+//   overflowing quotient, inf, NaN) it is recomputed unscaled.
+// Every product that can meet an addition (q * 2^-64 before p - u) is exact, so contraction cannot change those either.
+__host__ __device__ __forceinline__ void l4d_adam_elem(float& p, float& m, float& v, float g, float inv_scale, float beta1,
+                                                     float beta2, float eps, float step_size, float bc2_sqrt) {
+  g = g * inv_scale;
+  m = fmaf(beta1, m, fmaf(-beta1, g, g));
+  const float gsq = g * g;
+  v = fmaf(beta2, v, fmaf(-beta2, gsq, gsq));
+  const bool v_small = v < 0x1p64f;
+  const float root = sqrtf(v * (v_small ? 0x1p64f : 1.0f)) * (v_small ? 0x1p-32f : 1.0f);
+  const float den = root / bc2_sqrt + eps;
+  const float a = step_size * m;
+  const float q = (a * 0x1p64f) / den;
+  const float aq = fabsf(q);
+  float u = q * 0x1p-64f;
+  if (!((aq >= 0x1p-62f || aq == 0.0f) && aq <= 0x1.fffffep127f)) u = a / den;
+  p = p - u;
+}
+
 __global__ void __launch_bounds__(256) k_adam_flat(const __grid_constant__ AdamArgs A) {
+  const float bc1 = 1.0f - powf(A.beta1, A.step);
+  const float bc2_sqrt = sqrtf(1.0f - powf(A.beta2, A.step));
   for (unsigned long long c = blockIdx.x; c < A.n_chunks; c += gridDim.x) {
     const unsigned long long base = c * L4D_ADAM_CHUNK;
     int lo = 0, hi = A.n_seg - 1;                       // last segment with begin <= base (uniform per block)
@@ -45,28 +79,18 @@ __global__ void __launch_bounds__(256) k_adam_flat(const __grid_constant__ AdamA
       if (A.seg[mid].begin <= base) lo = mid; else hi = mid - 1;
     }
     const AdamSeg& s = A.seg[lo];
+    if (base < s.begin) continue;                       // chunk before the first segment: not covered
     const unsigned long long i = base + 4ull * threadIdx.x;
-    if (i >= s.end) continue;                           // alignment padding behind a tensor
+    if (i >= s.end) continue;                           // alignment padding behind a tensor, or a gap
     float4 p = *reinterpret_cast<const float4*>(A.p + i);
     float4 g = __ldcs(reinterpret_cast<const float4*>(A.g + i));
     float4 m = *reinterpret_cast<const float4*>(A.m + i);
     float4 v = *reinterpret_cast<const float4*>(A.v + i);
-    const float w = 1.0f - A.beta1, w2 = 1.0f - A.beta2;
-    const float step = s.lr / A.bc1;
-    // torch/aten fused_adam_utils.cuh adam_math (non-amsgrad, no weight decay): same operation order
-    // IEEE sqrtf / division branch into a slow path when an operand is subnormal, and second moments of rarely touched
-    // entries can be (g ~ 1e-20 => g^2 ~ 1e-40).  Scaling by exact powers of two keeps every operand normal and leaves all
-    // normal-range results bit-identical, so the kernel stays a pure stream (0.46 ms at L=16 for either bench loss).
-#define L4D_ADAM1(P, G, M, V)                                                                  \
-    {                                                                                          \
-      const float gg = (G) * A.inv_scale;                                                      \
-      M = fmaf(w, gg - (M), (M));                                                              \
-      V = A.beta2 * (V) + w2 * gg * gg;                                                        \
-      const float den = (sqrtf((V) * 1.8446744073709552e19f) * 2.3283064365386963e-10f) / A.bc2_sqrt + A.eps;   /* 2^64, 2^-32 */ \
-      P = (P) - ((step * (M)) * 1.8446744073709552e19f) / den * 5.421010862427522e-20f;        /* 2^64, 2^-64 */ \
-    }
-    L4D_ADAM1(p.x, g.x, m.x, v.x) L4D_ADAM1(p.y, g.y, m.y, v.y) L4D_ADAM1(p.z, g.z, m.z, v.z) L4D_ADAM1(p.w, g.w, m.w, v.w)
-#undef L4D_ADAM1
+    const float step_size = s.lr / bc1;
+    l4d_adam_elem(p.x, m.x, v.x, g.x, A.inv_scale, A.beta1, A.beta2, A.eps, step_size, bc2_sqrt);
+    l4d_adam_elem(p.y, m.y, v.y, g.y, A.inv_scale, A.beta1, A.beta2, A.eps, step_size, bc2_sqrt);
+    l4d_adam_elem(p.z, m.z, v.z, g.z, A.inv_scale, A.beta1, A.beta2, A.eps, step_size, bc2_sqrt);
+    l4d_adam_elem(p.w, m.w, v.w, g.w, A.inv_scale, A.beta1, A.beta2, A.eps, step_size, bc2_sqrt);
     *reinterpret_cast<float4*>(A.p + i) = p;
     *reinterpret_cast<float4*>(A.m + i) = m;
     *reinterpret_cast<float4*>(A.v + i) = v;

@@ -4,8 +4,10 @@ refresh of the fp16 hash tables the render kernels read (SURVEY.md 8(f) #4).
 Drop-in for the optimiser the reference builds in main_lidar4d.py:298-300
     optimizer = lambda model: torch.optim.Adam(model.get_params(opt.lr), betas=(0.9, 0.99), eps=1e-15)
 ->  optimizer = lambda model: lidar4d_b200.optim.Adam(model, model.get_params(opt.lr), betas=(0.9, 0.99), eps=1e-15)
-It is a torch.optim.Optimizer (param_groups / state_dict / LambdaLR / GradScaler.step work as usual); the arithmetic is
-torch's fused Adam (no weight decay, no amsgrad) in the same operation order.  There is no CPU path.
+It is a torch.optim.Optimizer (param_groups / state_dict / LambdaLR / GradScaler.step work as usual).  After every step
+the parameters and both moments are bit-identical to torch.optim.Adam(..., fused=True) of torch 2.11 (no weight decay, no
+amsgrad) on the same gradients, and the fp16 hash tables it refreshes are byte-identical to a from-scratch staging
+(tests/test_gpu_adam_exact.py).  The default, non-fused torch.optim.Adam rounds differently.  There is no CPU path.
 """
 from __future__ import annotations
 
