@@ -302,6 +302,40 @@ int    l4d_lidar_rays(const float* pose, float fov_up, float fov, uint32_t H, ui
 int    l4d_lidar_loss(const float* depth, const float* image2, const float* gt3, uint32_t n, float alpha_d, float alpha_r,
                       float alpha_i, float smooth, float* loss, float* g_depth, float* g_image2, void* stream);
 
+/* --- the rest of train_step: the patch losses (model/runner.py:278-369) and URF's line-of-sight loss (:255-276) ---------
+ * Inputs are fp32 device arrays; gt3[n, 3] = (raydrop m, intensity, depth) as for l4d_lidar_loss.  Both WRITE the loss to
+ * the device float *loss; sums are taken in a fixed order, so the same inputs give the same bits.  The backwards read the
+ * incoming gradient from the device float *g_loss and WRITE their gradient.  Null pointers and bad sizes: L4D_EINVAL.
+ * l4d_patch_loss: depth[n] read as n / (px*py) patches of px rows x py columns (get_lidar_rays' order), n % (px*py) == 0;
+ *   pred = depth*m/scale, gt_d = gt_depth*m/scale.  Writes the branch's summed loss (criterion `crit` = L4D_GRAD_*, terms
+ *   switched on by L4D_PATCH_* `flags`, weights alpha_*) and g_depth[n] = d loss / d depth.  px == 1 gives 0 and a zero
+ *   gradient, as the reference's `patch_size_x > 1`.  One launch (one CTA).
+ * l4d_patch_loss_backward: g_depth[n] = g_saved[n] * *g_loss (g_saved = the forward's g_depth).  One launch.
+ * l4d_los_loss: weights[n, S], z_vals[n, S], n*S < 2^32, the host `eps` of the reference (0.02 * 0.1^min(step/iters, 1)).
+ *   Writes 0.1*loss_empty + 0.1*loss_near; with no ray of gt depth > 0 that is the reference's inf / nan.  `work` =
+ *   l4d_los_work_bytes() bytes (L4D_ESIZE when smaller), kept for the backward.  Two launches; the second re-reads
+ *   [n, S] only when no sample lies outside its window (then max(distr) < its peak).
+ * l4d_los_loss_backward: g_weights[n, S] = d loss / d weights times *g_loss, with the forward's inputs and `work`. */
+#define L4D_GRAD_L1    0
+#define L4D_GRAD_MSE   1
+#define L4D_GRAD_HUBER 2
+#define L4D_GRAD_BCE   3
+#define L4D_GRAD_COS   4
+#define L4D_PATCH_SOBEL     1u   /* 3x3 Sobel with zero padding instead of finite differences */
+#define L4D_PATCH_GRAD      2u   /* grad_loss: the x-direction criterion, weight alpha_grad */
+#define L4D_PATCH_GRAD_NORM 4u   /* grad_norm_smooth: mean(exp(-dx)) + mean(exp(-dy)), weight alpha_grad_norm */
+#define L4D_PATCH_SPATIAL   8u   /* spatial_smooth: mean(dx^2) + mean(dy^2), weight alpha_spatial */
+#define L4D_PATCH_TV       16u   /* tv_loss: mean(dx) + mean(dy), weight alpha_tv */
+int    l4d_patch_loss(const float* depth, const float* gt3, uint32_t n, uint32_t px, uint32_t py, float scale, uint32_t crit,
+                      uint32_t flags, float alpha_grad, float alpha_grad_norm, float alpha_spatial, float alpha_tv, float* loss,
+                      float* g_depth, void* stream);
+int    l4d_patch_loss_backward(const float* g_saved, const float* g_loss, uint32_t n, float* g_depth, void* stream);
+size_t l4d_los_work_bytes(void);
+int    l4d_los_loss(const float* weights, const float* z_vals, const float* gt3, uint32_t n, uint32_t S, double eps,
+                    float* loss, void* work, size_t work_bytes, void* stream);
+int    l4d_los_loss_backward(const float* weights, const float* z_vals, const float* gt3, uint32_t n, uint32_t S, double eps,
+                             const void* work, const float* g_loss, float* g_weights, void* stream);
+
 /* --- range image <-> point cloud (utils/convert.py) and the point-cloud metric of PointsMeter (utils/metrics.py:229-279) ---
  * Images are H x W row-major with 1 <= H, W and H*W <= 2^31; otherwise, and for null required pointers, L4D_EINVAL.
  * l4d_pano_project = lidar_to_pano_with_intensities: points[n, stride] (stride 3, or 4 with the intensity in column 3) ->

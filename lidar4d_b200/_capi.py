@@ -152,6 +152,7 @@ EXPORTS = [
     "l4d_range_filter_work_bytes", "l4d_range_filter", "l4d_knn_mean_dist", "l4d_outlier_select_work_bytes",
     "l4d_outlier_select", "l4d_plane_scores", "l4d_plane_mask", "l4d_ground_split_work_bytes", "l4d_ground_split",
     "l4d_pose_transform",
+    "l4d_patch_loss", "l4d_patch_loss_backward", "l4d_los_work_bytes", "l4d_los_loss", "l4d_los_loss_backward",
 ]
 
 
@@ -218,6 +219,15 @@ def declare(lib, prefix: str = "l4d_", host_sim: bool = False):
         lib.l4d_lidar_rays.restype = C.c_int
         lib.l4d_lidar_loss.argtypes = [V, V, V, U32, C.c_float, C.c_float, C.c_float, C.c_float, V, V, V, V]
         lib.l4d_lidar_loss.restype = C.c_int
+        F = C.c_float
+        lib.l4d_patch_loss.argtypes = [V, V, U32, U32, U32, F, U32, U32, F, F, F, F, V, V, V]
+        lib.l4d_patch_loss_backward.argtypes = [V, V, U32, V, V]
+        lib.l4d_los_work_bytes.argtypes = []
+        lib.l4d_los_work_bytes.restype = SZ
+        lib.l4d_los_loss.argtypes = [V, V, V, U32, U32, C.c_double, V, V, SZ, V]
+        lib.l4d_los_loss_backward.argtypes = [V, V, V, U32, U32, C.c_double, V, V, V, V]
+        for n in ("patch_loss", "patch_loss_backward", "los_loss", "los_loss_backward"):
+            getattr(lib, f"l4d_{n}").restype = C.c_int
         lib.l4d_pano_project_work_bytes.argtypes = [U32, U32]
         lib.l4d_pano_project_work_bytes.restype = SZ
         lib.l4d_pano_project.argtypes = [V, U32, U32, C.c_double, C.c_double, U32, U32, C.c_float, V, V, V, SZ, V]

@@ -15,6 +15,7 @@
 #include "l4d_host.h"
 #include "l4d_tc.cuh"
 #include "l4d_optim.cuh"
+#include "l4d_losses.cuh"
 
 // =============================================================================
 // error plumbing
@@ -1719,6 +1720,73 @@ extern "C" int l4d_lidar_loss(const float* depth, const float* image, const floa
   int grid = nblk(n);
   if (grid > 4 * sm_count()) grid = 4 * sm_count();
   ++g_launches; k_lidar_loss<<<grid, 256, 0, (cudaStream_t)stream>>>(depth, image, gt, n, alpha_d, alpha_r, alpha_i, smooth, loss, g_depth, g_image);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+// =============================================================================
+// the patch losses and the line-of-sight loss of train_step (l4d_losses.cuh)
+// =============================================================================
+extern "C" int l4d_patch_loss(const float* depth, const float* gt, uint32_t n, uint32_t px, uint32_t py, float scale, uint32_t crit,
+                              uint32_t flags, float alpha_grad, float alpha_gn, float alpha_sp, float alpha_tv, float* loss,
+                              float* g_depth, void* stream) {
+  if (!depth || !gt || !loss || !g_depth) return l4d_fail(L4D_EINVAL, "l4d_patch_loss: null pointer");
+  if (px == 0 || py == 0 || n % (px * py) != 0) return l4d_fail(L4D_EINVAL, "l4d_patch_loss: n is not a multiple of px*py");
+  if (crit > L4D_GRAD_COS || (flags & ~31u)) return l4d_fail(L4D_EINVAL, "l4d_patch_loss: unknown criterion or flag");
+  const L4DPatchArgs a = l4d_patch_args(n, px, py, scale, crit, flags, alpha_grad, alpha_gn, alpha_sp, alpha_tv);
+  ++g_launches; k_patch_loss<<<1, L4D_PATCH_THREADS, 0, (cudaStream_t)stream>>>(depth, gt, n, a, loss, g_depth);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+extern "C" int l4d_patch_loss_backward(const float* g_saved, const float* g_loss, uint32_t n, float* g_depth, void* stream) {
+  if (!g_saved || !g_loss || !g_depth) return l4d_fail(L4D_EINVAL, "l4d_patch_loss_backward: null pointer");
+  if (n == 0) return L4D_OK;
+  int grid = nblk(n);
+  if (grid > 4 * sm_count()) grid = 4 * sm_count();
+  ++g_launches; k_loss_scale<<<grid, 256, 0, (cudaStream_t)stream>>>(g_saved, g_loss, n, g_depth);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+extern "C" size_t l4d_los_work_bytes(void) { return sizeof(L4DLosWork); }
+
+static int los_check(const float* w, const float* z, const float* gt, uint32_t n, uint32_t S, double eps, const char* who) {
+  if (!w || !z || !gt) return l4d_fail(L4D_EINVAL, "%s: null pointer", who);
+  if (n == 0 || S == 0 || (uint64_t)n * S >= (1ull << 32)) return l4d_fail(L4D_EINVAL, "%s: need 1 <= n, S and n*S < 2^32", who);
+  if (!(eps > 0.0)) return l4d_fail(L4D_EINVAL, "%s: eps must be positive", who);
+  return L4D_OK;
+}
+
+static int los_grid(uint32_t n, uint32_t S) {
+  const size_t b = ((size_t)n * S + L4D_LOS_THREADS - 1) / L4D_LOS_THREADS;
+  return (int)(b < L4D_LOS_BLOCKS ? b : L4D_LOS_BLOCKS);
+}
+
+extern "C" int l4d_los_loss(const float* w, const float* z, const float* gt, uint32_t n, uint32_t S, double eps, float* loss,
+                            void* work, size_t work_bytes, void* stream) {
+  if (int rc = los_check(w, z, gt, n, S, eps, "l4d_los_loss")) return rc;
+  if (!loss || !work) return l4d_fail(L4D_EINVAL, "l4d_los_loss: null pointer");
+  if (work_bytes < sizeof(L4DLosWork)) return l4d_fail(L4D_ESIZE, "l4d_los_loss: work buffer too small");
+  const L4DLosArgs a = l4d_los_args(eps);
+  const int grid = los_grid(n, S);
+  cudaStream_t st = (cudaStream_t)stream;
+  L4DLosWork* wk = (L4DLosWork*)work;
+  ++g_launches; k_los_partial<<<grid, L4D_LOS_THREADS, 0, st>>>(w, z, gt, n, S, a, wk);
+  L4D_CUDA(cudaGetLastError());
+  ++g_launches; k_los_finalize<<<1, 1024, 0, st>>>(w, z, gt, n, S, (uint32_t)grid, a, wk, loss);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+extern "C" int l4d_los_loss_backward(const float* w, const float* z, const float* gt, uint32_t n, uint32_t S, double eps,
+                                     const void* work, const float* g_loss, float* g_w, void* stream) {
+  if (int rc = los_check(w, z, gt, n, S, eps, "l4d_los_loss_backward")) return rc;
+  if (!work || !g_loss || !g_w) return l4d_fail(L4D_EINVAL, "l4d_los_loss_backward: null pointer");
+  const L4DLosArgs a = l4d_los_args(eps);
+  int grid = nblk((size_t)n * S);
+  if (grid > 8 * sm_count()) grid = 8 * sm_count();
+  ++g_launches; k_los_backward<<<grid, 256, 0, (cudaStream_t)stream>>>(w, z, gt, n, S, a, (const L4DLosWork*)work, g_loss, g_w);
   L4D_CUDA(cudaGetLastError());
   return L4D_OK;
 }

@@ -6,7 +6,15 @@ loss and, in the same pass, its gradient with respect to the render outputs (SUR
 
 equals  (alpha_d*L1(depth*m, gt_d*m) + alpha_r*MSE(raydrop, clamp(m, s, 1-s)) + alpha_i*MSE(intensity*m, gt_i*m)).sum()
 with m = gt[..., 0] (ray-drop mask), gt_i = gt[..., 1], gt_d = gt[..., 2] - the default criteria of main_lidar4d.py:63-66.
-No CPU path."""
+
+The rest of train_step (model/runner.py:255-369), each a CUDA op whose backward is one launch that reads the incoming
+gradient from device memory (a GradScaler-scaled backward needs no host sync):
+
+    loss = loss + line_of_sight_loss(out["weights"], out["z_vals"], gt, eps)        # --urf_loss
+    loss = loss + lidar_patch_loss(out["depth_lidar"], gt, **vars(opt))             # patch batches
+
+Inputs are taken in fp32 whatever the surrounding autocast (the reference's Sobel conv2d runs in fp16 under its fp16
+autocast; here it runs in fp32).  No CPU path."""
 from __future__ import annotations
 
 import torch
@@ -46,3 +54,116 @@ class _MainLoss(torch.autograd.Function):
 
 def lidar_main_loss(depth, image, gt, alpha_d=1.0, alpha_r=0.01, alpha_i=0.1, smooth=0.2):
     return _MainLoss.apply(depth, image, gt, alpha_d, alpha_r, alpha_i, smooth)
+
+
+GRAD_CRITERIA = {"l1": 0, "mse": 1, "huber": 2, "bce": 3, "cos": 4}      # L4D_GRAD_* (main_lidar4d.py:183-188)
+_SOBEL, _GRAD, _GRAD_NORM, _SPATIAL, _TV = 1, 2, 4, 8, 16                # L4D_PATCH_*
+
+
+def _stream(t):
+    return torch.cuda.current_stream(t.device).cuda_stream
+
+
+class _PatchLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, depth, gt, px, py, scale, crit, flags, a_grad, a_gn, a_sp, a_tv):
+        lib = _capi.load_library()
+        d = depth.detach().contiguous().view(-1).float()
+        g = gt.detach().contiguous().view(-1, 3).float()
+        n = d.numel()
+        loss = torch.empty((), device=d.device)
+        gd = torch.empty_like(d)
+        with torch.cuda.device(d.device):
+            rc = lib.l4d_patch_loss(d.data_ptr(), g.data_ptr(), n, px, py, float(scale), crit, flags, float(a_grad),
+                                    float(a_gn), float(a_sp), float(a_tv), loss.data_ptr(), gd.data_ptr(), _stream(d))
+        _capi.check(lib, rc, "l4d_patch_loss")
+        ctx.save_for_backward(gd)
+        ctx.shape = depth.shape
+        return loss
+
+    @staticmethod
+    def backward(ctx, gl):
+        (gd,) = ctx.saved_tensors
+        lib = _capi.load_library()
+        gl = gl.detach().float().contiguous()
+        out = torch.empty_like(gd)
+        with torch.cuda.device(gd.device):
+            rc = lib.l4d_patch_loss_backward(gd.data_ptr(), gl.data_ptr(), gd.numel(), out.data_ptr(), _stream(gd))
+        _capi.check(lib, rc, "l4d_patch_loss_backward")
+        return (out.view(ctx.shape),) + (None,) * 10
+
+
+def lidar_patch_loss(depth, gt, patch_size, scale, depth_grad_loss="l1", sobel_grad=False, grad_loss=True, alpha_grad=0.1,
+                     grad_norm_smooth=False, alpha_grad_norm=0.1, spatial_smooth=False, alpha_spatial=0.1, tv_loss=False,
+                     alpha_tv=0.1, **_):
+    """model/runner.py:278-369 as one launch: the depth-gradient loss of a patch batch and the optional smoothness terms,
+    summed, with d loss / d depth.  depth [.., n] (the render's depth_lidar), gt [.., n, 3] = (raydrop, intensity,
+    depth); the n rays are n / (px*py) patches of px rows x py columns, get_lidar_rays' order.  patch_size is an int,
+    [p] or [px, py] (runner.py:279-284); px == 1 gives 0, as in the reference.  Keyword names are the reference's opt
+    fields, so `**vars(opt)` can be passed (other keys are ignored)."""
+    if isinstance(patch_size, int):
+        px = py = patch_size
+    elif len(patch_size) == 1:
+        px = py = patch_size[0]
+    else:
+        px, py = patch_size
+    px, py = int(px), int(py)
+    if depth_grad_loss not in GRAD_CRITERIA:
+        raise ValueError(f"depth_grad_loss must be one of {sorted(GRAD_CRITERIA)}, got {depth_grad_loss!r}")
+    if not (depth.is_cuda and gt.is_cuda):
+        raise RuntimeError("lidar_patch_loss runs on CUDA only (no CPU fallback)")
+    n = depth.numel()
+    if gt.numel() != 3 * n or gt.shape[-1] != 3:
+        raise ValueError("depth [.., n] and gt [.., n, 3] must describe the same rays")
+    if px < 1 or py < 1 or n % (px * py):
+        raise ValueError(f"{n} rays are not a whole number of {px}x{py} patches")
+    flags = ((_SOBEL if sobel_grad else 0) | (_GRAD if grad_loss else 0) | (_GRAD_NORM if grad_norm_smooth else 0)
+             | (_SPATIAL if spatial_smooth else 0) | (_TV if tv_loss else 0))
+    return _PatchLoss.apply(depth, gt, px, py, scale, GRAD_CRITERIA[depth_grad_loss], flags, alpha_grad, alpha_grad_norm,
+                            alpha_spatial, alpha_tv)
+
+
+class _LineOfSightLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, weights, z_vals, gt, eps):
+        lib = _capi.load_library()
+        n, S = weights.shape
+        w = weights.detach().contiguous().float()
+        z = z_vals.detach().contiguous().float()
+        g = gt.detach().contiguous().view(-1, 3).float()
+        loss = torch.empty((), device=w.device)
+        work = torch.empty(lib.l4d_los_work_bytes(), dtype=torch.uint8, device=w.device)
+        with torch.cuda.device(w.device):
+            rc = lib.l4d_los_loss(w.data_ptr(), z.data_ptr(), g.data_ptr(), n, S, float(eps), loss.data_ptr(),
+                                  work.data_ptr(), work.numel(), _stream(w))
+        _capi.check(lib, rc, "l4d_los_loss")
+        ctx.save_for_backward(w, z, g, work)
+        ctx.eps = float(eps)
+        return loss
+
+    @staticmethod
+    def backward(ctx, gl):
+        w, z, g, work = ctx.saved_tensors
+        lib = _capi.load_library()
+        gl = gl.detach().float().contiguous()
+        gw = torch.empty_like(w)
+        with torch.cuda.device(w.device):
+            rc = lib.l4d_los_loss_backward(w.data_ptr(), z.data_ptr(), g.data_ptr(), w.shape[0], w.shape[1], ctx.eps,
+                                           work.data_ptr(), gl.data_ptr(), gw.data_ptr(), _stream(w))
+        _capi.check(lib, rc, "l4d_los_loss_backward")
+        return gw, None, None, None
+
+
+def line_of_sight_loss(weights, z_vals, gt, eps):
+    """model/runner.py:255-276 (URF's line-of-sight loss): 0.1 * loss_empty + 0.1 * loss_near over weights / z_vals
+    [n, S] (the render's outputs) and gt [.., n, 3], with the caller's eps = 0.02 * 0.1 ** min(step / iters, 1).
+    Differentiable in weights.  With no ray of gt depth > 0 the value is the reference's inf / nan."""
+    if not (weights.is_cuda and z_vals.is_cuda and gt.is_cuda):
+        raise RuntimeError("line_of_sight_loss runs on CUDA only (no CPU fallback)")
+    if weights.dim() != 2 or z_vals.shape != weights.shape:
+        raise ValueError("weights and z_vals must both be [n, S]")
+    if gt.numel() != 3 * weights.shape[0] or gt.shape[-1] != 3:
+        raise ValueError("gt must be [.., n, 3] for the n rays of weights")
+    if weights.numel() == 0:
+        raise ValueError("line_of_sight_loss of an empty batch (the reference's distr.max() raises too)")
+    return _LineOfSightLoss.apply(weights, z_vals, gt, eps)
