@@ -336,6 +336,41 @@ int    l4d_los_loss(const float* weights, const float* z_vals, const float* gt3,
 int    l4d_los_loss_backward(const float* weights, const float* z_vals, const float* gt3, uint32_t n, uint32_t S, double eps,
                              const void* work, const float* g_loss, float* g_weights, void* stream);
 
+/* --- exact nearest-neighbour search through a uniform grid, and the flow loss of train_step (model/runner.py:222-253) -----
+ * For clouds that are searched many times (every optimiser step of the flow loss).  b = 1 only; xyz[n, 3] fp32, 1 <= n < 2^31.
+ * l4d_nn_grid_build indexes a cloud into `grid` (l4d_nn_grid_bytes(n) bytes, 16-byte aligned, the caller's; it holds a copy
+ *   of the points, so xyz may be released) with `work` = l4d_nn_grid_work_bytes(n) scratch bytes (L4D_ESIZE when smaller).
+ *   Five launches, no device-to-host read.  Points with a non-finite coordinate are left out (they can never be nearest).
+ * l4d_nn_grid_query: for q[nq, 3], dist[nq] / idx[nq] = squared distance to, and ORIGINAL index of, the nearest indexed
+ *   point - bit for bit what l4d_chamfer_forward returns for (q, xyz), the smallest index on ties, (+inf, 0) for a query
+ *   with a non-finite coordinate or a cloud without a finite point.  `n` is the n of the build.  dist may be NULL when
+ *   sum_parts is given: sum_parts[L4D_FLOW_PARTS] doubles receive per-CTA sums of dist (entries beyond the launch's CTAs
+ *   are not written: zero them first).  One launch.
+ * The flow loss, for pc[n, 3], flow6[n, 6] = (forward | backward) flow of pc, and one neighbouring frame's cloud target[m, 3]
+ * with its index `grid`:
+ *   l4d_flow_warp_query: warped[n, 3] = pc + flow6[:, 3 dir .. 3 dir + 2] * step, idx1[n] = nearest target of every warped
+ *     point, sum_parts as above.  One launch.  The caller then indexes `warped` (l4d_nn_grid_build) and queries it with
+ *     `target` (l4d_nn_grid_query) for idx2[m].
+ *   l4d_flow_term_backward ACCUMULATES d (0.5 (sum dist1 + sum dist2)) / d flow6 times the device float *g_loss into
+ *     g_flow6[n, 6] (columns 3 dir .. 3 dir + 2).  One launch; the target gets no gradient.
+ *   l4d_flow_ground: per-CTA sums of |flow6| over [n, 6] into sum_parts[L4D_FLOW_PARTS]; l4d_flow_ground_backward WRITES
+ *     g_flow6 = 0.001 sign(flow6) *g_loss.
+ *   l4d_flow_loss_finish: *loss = 0.5 * sum(sum_parts[0 .. n_chamfer)) + 0.001 * sum(sum_parts[n_chamfer .. + n_ground)),
+ *     in double and in a fixed order: the same inputs give the same bits. */
+#define L4D_FLOW_PARTS 2048
+size_t l4d_nn_grid_bytes(uint32_t n);
+size_t l4d_nn_grid_work_bytes(uint32_t n);
+int    l4d_nn_grid_build(const float* xyz, uint32_t n, void* grid, size_t grid_bytes, void* work, size_t work_bytes, void* stream);
+int    l4d_nn_grid_query(const void* grid, size_t grid_bytes, uint32_t n, const float* q, uint32_t nq, float* dist_or_null,
+                         int32_t* idx, double* sum_parts_or_null, void* stream);
+int    l4d_flow_warp_query(const float* pc, const float* flow6, uint32_t n, uint32_t dir, float step, const void* grid,
+                           size_t grid_bytes, uint32_t m, float* warped, int32_t* idx1, double* sum_parts, void* stream);
+int    l4d_flow_term_backward(const float* warped, uint32_t n, const float* target, uint32_t m, const int32_t* idx1,
+                              const int32_t* idx2, uint32_t dir, float step, const float* g_loss, float* g_flow6, void* stream);
+int    l4d_flow_ground(const float* flow6, uint32_t n, double* sum_parts, void* stream);
+int    l4d_flow_ground_backward(const float* flow6, uint32_t n, const float* g_loss, float* g_flow6, void* stream);
+int    l4d_flow_loss_finish(const double* sum_parts, uint32_t n_chamfer, uint32_t n_ground, float* loss, void* stream);
+
 /* --- range image <-> point cloud (utils/convert.py) and the point-cloud metric of PointsMeter (utils/metrics.py:229-279) ---
  * Images are H x W row-major with 1 <= H, W and H*W <= 2^31; otherwise, and for null required pointers, L4D_EINVAL.
  * l4d_pano_project = lidar_to_pano_with_intensities: points[n, stride] (stride 3, or 4 with the intensity in column 3) ->

@@ -16,6 +16,7 @@ MAX_TIME_SLICES = 16
 ABI_VERSION = 1
 STAGE_TABLES, STAGE_SMALL = 1, 2        # l4d_stage_params_ex `what`
 ADAM_CHUNK, ADAM_MAX_SEGMENTS = 1024, 64
+FLOW_PARTS = 2048                       # L4D_FLOW_PARTS: per-launch slots of the flow loss's partial sums
 
 c_float_p = C.POINTER(C.c_float)
 
@@ -153,6 +154,8 @@ EXPORTS = [
     "l4d_outlier_select", "l4d_plane_scores", "l4d_plane_mask", "l4d_ground_split_work_bytes", "l4d_ground_split",
     "l4d_pose_transform",
     "l4d_patch_loss", "l4d_patch_loss_backward", "l4d_los_work_bytes", "l4d_los_loss", "l4d_los_loss_backward",
+    "l4d_nn_grid_bytes", "l4d_nn_grid_work_bytes", "l4d_nn_grid_build", "l4d_nn_grid_query", "l4d_flow_warp_query",
+    "l4d_flow_term_backward", "l4d_flow_ground", "l4d_flow_ground_backward", "l4d_flow_loss_finish",
 ]
 
 
@@ -227,6 +230,19 @@ def declare(lib, prefix: str = "l4d_", host_sim: bool = False):
         lib.l4d_los_loss.argtypes = [V, V, V, U32, U32, C.c_double, V, V, SZ, V]
         lib.l4d_los_loss_backward.argtypes = [V, V, V, U32, U32, C.c_double, V, V, V, V]
         for n in ("patch_loss", "patch_loss_backward", "los_loss", "los_loss_backward"):
+            getattr(lib, f"l4d_{n}").restype = C.c_int
+        for n in ("nn_grid_bytes", "nn_grid_work_bytes"):
+            getattr(lib, f"l4d_{n}").argtypes = [U32]
+            getattr(lib, f"l4d_{n}").restype = SZ
+        lib.l4d_nn_grid_build.argtypes = [V, U32, V, SZ, V, SZ, V]
+        lib.l4d_nn_grid_query.argtypes = [V, SZ, U32, V, U32, V, V, V, V]
+        lib.l4d_flow_warp_query.argtypes = [V, V, U32, U32, F, V, SZ, U32, V, V, V, V]
+        lib.l4d_flow_term_backward.argtypes = [V, U32, V, U32, V, V, U32, F, V, V, V]
+        lib.l4d_flow_ground.argtypes = [V, U32, V, V]
+        lib.l4d_flow_ground_backward.argtypes = [V, U32, V, V, V]
+        lib.l4d_flow_loss_finish.argtypes = [V, U32, U32, V, V]
+        for n in ("nn_grid_build", "nn_grid_query", "flow_warp_query", "flow_term_backward", "flow_ground",
+                  "flow_ground_backward", "flow_loss_finish"):
             getattr(lib, f"l4d_{n}").restype = C.c_int
         lib.l4d_pano_project_work_bytes.argtypes = [U32, U32]
         lib.l4d_pano_project_work_bytes.restype = SZ

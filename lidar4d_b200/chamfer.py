@@ -75,3 +75,93 @@ class chamfer_3DFunction(Function):
 class chamfer_3DDist(nn.Module):
     def forward(self, input1, input2):
         return chamfer_3DFunction.apply(input1.contiguous(), input2.contiguous())
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# the same op through a uniform-grid index: for clouds that are searched many times (the flow loss's frame clouds)
+# ----------------------------------------------------------------------------------------------------------------------
+def _stream(t):
+    return torch.cuda.current_stream(t.device).cuda_stream
+
+
+class PointGrid:
+    """A cloud ``points[n, 3]`` (or [1, n, 3]) on the GPU with its nearest-neighbour index (l4d_nn_grid_build): built once,
+    queried by ``chamfer_3DGrid`` and by the flow loss.  The index holds its own copy of the coordinates; ``points`` is the
+    float32 cloud in its original order.  b = 1 only."""
+
+    def __init__(self, points):
+        if not isinstance(points, torch.Tensor) or not points.is_cuda:
+            raise RuntimeError("PointGrid needs a CUDA tensor (no CPU fallback)")
+        if points.dim() == 3 and points.shape[0] != 1:
+            raise ValueError("PointGrid indexes one cloud (b = 1)")
+        if points.dim() not in (2, 3) or points.shape[-1] != 3:
+            raise ValueError(f"PointGrid: expected [n, 3] or [1, n, 3], got {tuple(points.shape)}")
+        pts = points.detach().reshape(-1, 3).contiguous().float()
+        if pts.shape[0] == 0:
+            raise ValueError("PointGrid: empty point cloud")
+        lib = _capi.load_library()
+        self.points = pts
+        self.n = pts.shape[0]
+        self.nbytes = lib.l4d_nn_grid_bytes(self.n)
+        self.grid = torch.empty(self.nbytes, dtype=torch.uint8, device=pts.device)
+        nwork = lib.l4d_nn_grid_work_bytes(self.n)
+        work = torch.empty(nwork, dtype=torch.uint8, device=pts.device)
+        with torch.cuda.device(pts.device):
+            rc = lib.l4d_nn_grid_build(pts.data_ptr(), self.n, self.grid.data_ptr(), self.nbytes, work.data_ptr(), nwork,
+                                       _stream(pts))
+        _capi.check(lib, rc, "l4d_nn_grid_build")
+
+    def query(self, q, sum_parts=None, want_dist=True):
+        """q [nq, 3] float32 contiguous -> (dist [nq] or None, idx [nq] int32): the nearest point of this cloud."""
+        lib = _capi.load_library()
+        nq = q.shape[0]
+        dist = torch.empty(nq, device=q.device) if want_dist else None
+        idx = torch.empty(nq, dtype=torch.int32, device=q.device)
+        with torch.cuda.device(q.device):
+            rc = lib.l4d_nn_grid_query(self.grid.data_ptr(), self.nbytes, self.n, q.data_ptr(), nq,
+                                       dist.data_ptr() if want_dist else None, idx.data_ptr(),
+                                       sum_parts.data_ptr() if sum_parts is not None else None, _stream(q))
+        _capi.check(lib, rc, "l4d_nn_grid_query")
+        return dist, idx
+
+
+class _Chamfer3DGridFunction(Function):
+    @staticmethod
+    def forward(ctx, xyz1, xyz2, grid1, grid2):
+        ctx.in_dtypes = (xyz1.dtype, xyz2.dtype)
+        xyz1 = xyz1.contiguous().float()
+        xyz2 = xyz2.contiguous().float()
+        grid1 = grid1 if grid1 is not None else PointGrid(xyz1)
+        grid2 = grid2 if grid2 is not None else PointGrid(xyz2)
+        dist1, idx1 = grid2.query(xyz1[0])
+        dist2, idx2 = grid1.query(xyz2[0])
+        dist1, dist2, idx1, idx2 = dist1[None], dist2[None], idx1[None], idx2[None]
+        ctx.save_for_backward(xyz1, xyz2, idx1, idx2)
+        ctx.mark_non_differentiable(idx1, idx2)
+        return dist1, dist2, idx1, idx2
+
+    @staticmethod
+    def backward(ctx, graddist1, graddist2, gradidx1, gradidx2):
+        return chamfer_3DFunction.backward(ctx, graddist1, graddist2, gradidx1, gradidx2) + (None, None)
+
+
+class chamfer_3DGrid(nn.Module):
+    """``chamfer_3DDist`` with the search done through a uniform grid: same call, same four outputs, bit for bit, same
+    backward (l4d_chamfer_backward on the returned indices).  Each argument is a [1, N, 3] tensor, indexed on the fly, or a
+    prebuilt ``PointGrid`` (no gradient flows to a PointGrid)."""
+
+    def forward(self, input1, input2):
+        grids, clouds = [], []
+        for name, x in (("xyz1", input1), ("xyz2", input2)):
+            if isinstance(x, PointGrid):
+                grids.append(x)
+                clouds.append(x.points[None])
+            else:
+                _check_cloud(x, name)
+                if x.shape[0] != 1:
+                    raise ValueError("chamfer_3DGrid takes one cloud per side (b = 1); chamfer_3DDist handles batches")
+                grids.append(None)
+                clouds.append(x.contiguous())
+        if clouds[0].device != clouds[1].device:
+            raise ValueError("the two clouds are on different devices")
+        return _Chamfer3DGridFunction.apply(clouds[0], clouds[1], grids[0], grids[1])

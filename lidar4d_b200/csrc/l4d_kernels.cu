@@ -16,6 +16,7 @@
 #include "l4d_tc.cuh"
 #include "l4d_optim.cuh"
 #include "l4d_losses.cuh"
+#include "l4d_nngrid.cuh"
 
 // =============================================================================
 // error plumbing
@@ -1787,6 +1788,111 @@ extern "C" int l4d_los_loss_backward(const float* w, const float* z, const float
   int grid = nblk((size_t)n * S);
   if (grid > 8 * sm_count()) grid = 8 * sm_count();
   ++g_launches; k_los_backward<<<grid, 256, 0, (cudaStream_t)stream>>>(w, z, gt, n, S, a, (const L4DLosWork*)work, g_loss, g_w);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+// =============================================================================
+// exact grid nearest-neighbour search and the flow loss of train_step (l4d_nngrid.cuh)
+// =============================================================================
+extern "C" size_t l4d_nn_grid_bytes(uint32_t n) { return l4d_nng_layout(n).total; }
+extern "C" size_t l4d_nn_grid_work_bytes(uint32_t n) { return l4d_nng_work(n).total; }
+
+static int nng_grid(size_t n, int threads, int cap) {
+  const int b = nblk(n, threads);
+  return b < cap ? (b < 1 ? 1 : b) : cap;
+}
+
+extern "C" int l4d_nn_grid_build(const float* xyz, uint32_t n, void* grid, size_t grid_bytes, void* work, size_t work_bytes,
+                                 void* stream) {
+  if (!xyz || !grid || !work) return l4d_fail(L4D_EINVAL, "l4d_nn_grid_build: null pointer");
+  if (n == 0 || n >= (1u << 31)) return l4d_fail(L4D_EINVAL, "l4d_nn_grid_build: need 1 <= n < 2^31");
+  const L4DNNGLayout L = l4d_nng_layout(n);
+  const L4DNNGWork W = l4d_nng_work(n);
+  if (grid_bytes < L.total) return l4d_fail(L4D_ESIZE, "l4d_nn_grid_build: grid buffer too small");
+  if (work_bytes < W.total) return l4d_fail(L4D_ESIZE, "l4d_nn_grid_build: work buffer too small");
+  if (((uintptr_t)grid | (uintptr_t)work) & 15) return l4d_fail(L4D_EINVAL, "l4d_nn_grid_build: buffers must be 16-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned char* g = reinterpret_cast<unsigned char*>(grid);
+  unsigned char* w = reinterpret_cast<unsigned char*>(work);
+  L4DNNGHeader* H = reinterpret_cast<L4DNNGHeader*>(g);
+  uint32_t* start = reinterpret_cast<uint32_t*>(g + L.start);
+  float* part = reinterpret_cast<float*>(w + W.bbox);
+  uint32_t* cell_of = reinterpret_cast<uint32_t*>(w + W.cell_of);
+  uint32_t* cursor = reinterpret_cast<uint32_t*>(w + W.cursor);
+  const int bb = nng_grid((size_t)L.budget + 1 > n ? (size_t)L.budget + 1 : n, 256, L4D_NNG_BBOX_BLOCKS);
+  const int pb = nng_grid(n, 256, 8 * sm_count());
+  ++g_launches; k_nng_bbox<<<bb, 256, 0, st>>>(xyz, n, part, start, L.budget + 1);
+  ++g_launches; k_nng_geometry<<<1, 32, 0, st>>>(part, (uint32_t)bb, L.budget, H);
+  ++g_launches; k_nng_count<<<pb, 256, 0, st>>>(xyz, n, H, cell_of, start);
+  ++g_launches; k_nng_scan<<<1, 1024, 0, st>>>(H, start, cursor);
+  ++g_launches; k_nng_scatter<<<pb, 256, 0, st>>>(xyz, n, cell_of, cursor, reinterpret_cast<float4*>(g + L.pts));
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+static int nng_query_check(const void* grid, size_t grid_bytes, uint32_t n, const float* q, uint32_t nq, const int32_t* idx,
+                           const char* who) {
+  if (!grid || !q || !idx) return l4d_fail(L4D_EINVAL, "%s: null pointer", who);
+  if (n == 0 || n >= (1u << 31) || nq == 0 || nq >= (1u << 31)) return l4d_fail(L4D_EINVAL, "%s: need 1 <= n, nq < 2^31", who);
+  if (grid_bytes < l4d_nng_layout(n).total) return l4d_fail(L4D_ESIZE, "%s: grid buffer too small for n", who);
+  return L4D_OK;
+}
+
+extern "C" int l4d_nn_grid_query(const void* grid, size_t grid_bytes, uint32_t n, const float* q, uint32_t nq, float* dist,
+                                 int32_t* idx, double* sum_parts, void* stream) {
+  if (int rc = nng_query_check(grid, grid_bytes, n, q, nq, idx, "l4d_nn_grid_query")) return rc;
+  if (!dist && !sum_parts) return l4d_fail(L4D_EINVAL, "l4d_nn_grid_query: neither dist nor sum_parts given");
+  ++g_launches;
+  k_nng_query<false><<<nng_grid(nq, L4D_NNG_QT, L4D_FLOW_PARTS), L4D_NNG_QT, 0, (cudaStream_t)stream>>>(
+      reinterpret_cast<const unsigned char*>(grid), l4d_nng_layout(n), q, nullptr, 0, 0.f, nullptr, nq, dist, idx, sum_parts);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+extern "C" int l4d_flow_warp_query(const float* pc, const float* flow6, uint32_t n, uint32_t dir, float step, const void* grid,
+                                   size_t grid_bytes, uint32_t m, float* warped, int32_t* idx1, double* sum_parts, void* stream) {
+  if (int rc = nng_query_check(grid, grid_bytes, m, pc, n, idx1, "l4d_flow_warp_query")) return rc;
+  if (!flow6 || !warped || !sum_parts || dir > 1) return l4d_fail(L4D_EINVAL, "l4d_flow_warp_query: null pointer or dir > 1");
+  ++g_launches;
+  k_nng_query<true><<<nng_grid(n, L4D_NNG_QT, L4D_FLOW_PARTS), L4D_NNG_QT, 0, (cudaStream_t)stream>>>(
+      reinterpret_cast<const unsigned char*>(grid), l4d_nng_layout(m), pc, flow6, 3 * dir, step, warped, n, nullptr, idx1, sum_parts);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+extern "C" int l4d_flow_term_backward(const float* warped, uint32_t n, const float* target, uint32_t m, const int32_t* idx1,
+                                      const int32_t* idx2, uint32_t dir, float step, const float* g_loss, float* g_flow6,
+                                      void* stream) {
+  if (!warped || !target || !idx1 || !idx2 || !g_loss || !g_flow6 || dir > 1) return l4d_fail(L4D_EINVAL, "l4d_flow_term_backward: null pointer or dir > 1");
+  if (n == 0 || m == 0) return l4d_fail(L4D_EINVAL, "l4d_flow_term_backward: empty point cloud");
+  ++g_launches;
+  k_flow_term_bwd<<<nng_grid(n > m ? n : m, 256, 8 * sm_count()), 256, 0, (cudaStream_t)stream>>>(warped, n, target, m, idx1, idx2,
+                                                                                                3 * dir, step, g_loss, g_flow6);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+extern "C" int l4d_flow_ground(const float* flow6, uint32_t n, double* sum_parts, void* stream) {
+  if (!flow6 || !sum_parts) return l4d_fail(L4D_EINVAL, "l4d_flow_ground: null pointer");
+  if (n >= (1u << 29)) return l4d_fail(L4D_EINVAL, "l4d_flow_ground: n too large");
+  ++g_launches; k_flow_ground<<<nng_grid((size_t)n * 6, 256, L4D_FLOW_PARTS), 256, 0, (cudaStream_t)stream>>>(flow6, n * 6, sum_parts);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+extern "C" int l4d_flow_ground_backward(const float* flow6, uint32_t n, const float* g_loss, float* g_flow6, void* stream) {
+  if (!flow6 || !g_loss || !g_flow6) return l4d_fail(L4D_EINVAL, "l4d_flow_ground_backward: null pointer");
+  if (n >= (1u << 29)) return l4d_fail(L4D_EINVAL, "l4d_flow_ground_backward: n too large");
+  if (n == 0) return L4D_OK;
+  ++g_launches; k_flow_ground_bwd<<<nng_grid((size_t)n * 6, 256, 8 * sm_count()), 256, 0, (cudaStream_t)stream>>>(flow6, n * 6, g_loss, g_flow6);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+extern "C" int l4d_flow_loss_finish(const double* sum_parts, uint32_t n_chamfer, uint32_t n_ground, float* loss, void* stream) {
+  if (!sum_parts || !loss) return l4d_fail(L4D_EINVAL, "l4d_flow_loss_finish: null pointer");
+  ++g_launches; k_flow_finish<<<1, 1024, 0, (cudaStream_t)stream>>>(sum_parts, n_chamfer, n_ground, loss);
   L4D_CUDA(cudaGetLastError());
   return L4D_OK;
 }

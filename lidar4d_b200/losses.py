@@ -167,3 +167,124 @@ def line_of_sight_loss(weights, z_vals, gt, eps):
     if weights.numel() == 0:
         raise ValueError("line_of_sight_loss of an empty batch (the reference's distr.max() raises too)")
     return _LineOfSightLoss.apply(weights, z_vals, gt, eps)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# flow loss (model/runner.py:222-253)
+# ----------------------------------------------------------------------------------------------------------------------
+class FlowClouds:
+    """Every frame's cloud and ground cloud on the device, uploaded once and converted as the reference converts them
+    every step (float64 NumPy -> float32), each frame cloud with its nearest-neighbour index (chamfer.PointGrid).
+    Build it once after ``process_pointcloud``; keys are the reference's (``f"{frame_idx}"``)."""
+
+    def __init__(self, pc_list, pc_ground_list, device):
+        from .chamfer import PointGrid
+        device = torch.device(device)
+        if device.type != "cuda":
+            raise RuntimeError("FlowClouds lives on a CUDA device (no CPU fallback)")
+
+        def up(a):
+            a = a if isinstance(a, torch.Tensor) else torch.from_numpy(a)
+            return a.to(device).float().contiguous().view(-1, 3)
+
+        self.device = device
+        self.grids = {k: PointGrid(up(v)) for k, v in pc_list.items()}
+        self.ground = {k: up(v) for k, v in pc_ground_list.items()}
+
+
+class _FlowLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, flow, ground_flow, cur, terms):
+        """flow [n, 6] of the current frame's cloud `cur` (a PointGrid), ground_flow [g, 6]; terms = [(dir, step, PointGrid
+        of the neighbouring frame)].  Per term: warp + query of the static index, index of the warped cloud, query of it."""
+        from .chamfer import PointGrid
+        lib = _capi.load_library()
+        P = _capi.FLOW_PARTS
+        fl = flow.detach().contiguous().float()
+        gf = ground_flow.detach().contiguous().float()
+        dev, n = fl.device, cur.n
+        if fl.shape != (n, 6) or gf.dim() != 2 or gf.shape[1] != 6:
+            raise ValueError("flow must be [n, 6] for the n points of the frame's cloud, ground_flow [g, 6]")
+        parts = torch.zeros((2 * len(terms) + 1) * P, dtype=torch.float64, device=dev)
+        saved = []
+        with torch.cuda.device(dev):
+            for i, (d, step, tgt) in enumerate(terms):
+                warped = torch.empty(n, 3, device=dev)
+                idx1 = torch.empty(n, dtype=torch.int32, device=dev)
+                rc = lib.l4d_flow_warp_query(cur.points.data_ptr(), fl.data_ptr(), n, d, float(step), tgt.grid.data_ptr(),
+                                             tgt.nbytes, tgt.n, warped.data_ptr(), idx1.data_ptr(),
+                                             parts[2 * i * P:].data_ptr(), _stream(fl))
+                _capi.check(lib, rc, "l4d_flow_warp_query")
+                _, idx2 = PointGrid(warped).query(tgt.points, sum_parts=parts[(2 * i + 1) * P:], want_dist=False)
+                saved += [warped, idx1, idx2]
+            if gf.shape[0]:
+                rc = lib.l4d_flow_ground(gf.data_ptr(), gf.shape[0], parts[2 * len(terms) * P:].data_ptr(), _stream(fl))
+                _capi.check(lib, rc, "l4d_flow_ground")
+            loss = torch.empty((), device=dev)
+            rc = lib.l4d_flow_loss_finish(parts.data_ptr(), 2 * len(terms) * P, P, loss.data_ptr(), _stream(fl))
+            _capi.check(lib, rc, "l4d_flow_loss_finish")
+        ctx.save_for_backward(gf, *saved)
+        ctx.terms = terms
+        ctx.in_dtypes = (flow.dtype, ground_flow.dtype)
+        return loss
+
+    @staticmethod
+    def backward(ctx, gl):
+        gf, *saved = ctx.saved_tensors
+        lib = _capi.load_library()
+        gl = gl.detach().float().contiguous()
+        n = saved[0].shape[0] if saved else 0
+        g_flow = torch.zeros(n, 6, device=gf.device) if saved else None
+        g_ground = torch.empty_like(gf)
+        with torch.cuda.device(gf.device):
+            for i, (d, step, tgt) in enumerate(ctx.terms):
+                warped, idx1, idx2 = saved[3 * i:3 * i + 3]
+                rc = lib.l4d_flow_term_backward(warped.data_ptr(), n, tgt.points.data_ptr(), tgt.n, idx1.data_ptr(),
+                                                idx2.data_ptr(), d, float(step), gl.data_ptr(), g_flow.data_ptr(), _stream(gf))
+                _capi.check(lib, rc, "l4d_flow_term_backward")
+            rc = lib.l4d_flow_ground_backward(gf.data_ptr(), gf.shape[0], gl.data_ptr(), g_ground.data_ptr(), _stream(gf))
+            _capi.check(lib, rc, "l4d_flow_ground_backward")
+        if g_flow is not None:
+            g_flow = g_flow.to(ctx.in_dtypes[0])
+        return g_flow, g_ground.to(ctx.in_dtypes[1]), None, None
+
+
+def flow_loss_terms(clouds, frame_idx):
+    """The chamfer terms of frame `frame_idx` in the reference's order: [(0 forward | 1 backward, step, PointGrid)] for
+    step in (1, 2) and each direction whose frame exists."""
+    terms = []
+    for step in (1, 2):
+        for d, sign in ((0, +1), (1, -1)):
+            k = f"{frame_idx + sign * step}"
+            if k in clouds.grids:
+                terms.append((d, step, clouds.grids[k]))
+    return terms
+
+
+def flow_loss_from_flows(clouds, frame_idx, flow, ground_flow):
+    """The flow loss given the two flow predictions as [n, 6] = (forward | backward) tensors: everything of
+    model/runner.py:222-253 after the ``model.flow`` calls.  No device-to-host read, forward or backward."""
+    cur = clouds.grids[f"{frame_idx}"]
+    if flow.shape[0] != cur.n:
+        raise ValueError("flow must be [n, 6] for the n points of the frame's cloud")
+    return _FlowLoss.apply(flow, ground_flow, cur, flow_loss_terms(clouds, frame_idx))
+
+
+def lidar_flow_loss(model, clouds, time, num_frames, ground_time=None):
+    """model/runner.py:222-253: with pc the cloud of frame int(time * (num_frames - 1)) and flow = model.flow(pc, time),
+    for step in (1, 2) and each direction whose frame exists, 0.5 * (sum dist1 + sum dist2) between pc + flow_dir * step and
+    that frame's cloud, plus 0.001 * (sum |forward| + sum |backward|) of model.flow(ground, tau).  tau is drawn as the
+    reference draws it (``torch.rand(1).to(time)``), so the CPU generator ends in the reference's state; `ground_time`
+    overrides it.  A frame without a cloud raises KeyError.
+
+        clouds = FlowClouds(trainer.pc_list, trainer.pc_ground_list, device)      # once, after process_pointcloud
+        loss = loss + lidar_flow_loss(model, clouds, time_lidar, num_frames=opt.num_frames)
+    """
+    frame_idx = int(time * (num_frames - 1))
+    cur = clouds.grids[f"{frame_idx}"]
+    fl = model.flow(cur.points, time)
+    ground = clouds.ground[f"{frame_idx}"]
+    tau = torch.rand(1).to(time) if ground_time is None else ground_time
+    zf = model.flow(ground, tau)
+    return flow_loss_from_flows(clouds, frame_idx, torch.cat([fl["forward"], fl["backward"]], 1),
+                                torch.cat([zf["forward"], zf["backward"]], 1))
