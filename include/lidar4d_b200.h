@@ -393,6 +393,25 @@ int    l4d_pano_unproject(const float* pano, const float* intensities_or_null, u
                           float* out, uint32_t* count, void* work, size_t work_bytes, void* stream);
 int    l4d_point_metrics(const float* dist1, uint32_t n, const float* dist2, uint32_t m, float thr, float* out, void* stream);
 
+/* --- the depth / intensity / ray-drop meters (utils/metrics.py DepthMeter, IntensityMeter, RaydropMeter) -------------
+ * Results are WRITTEN as doubles to device memory; no host read, the caller's stream, and sums in a fixed order, so the
+ * same inputs give the same bits.  Null pointers and bad sizes: L4D_EINVAL.
+ * l4d_image_metrics = compute_depth_errors / compute_intensity_errors on fp32 pred, gt [H, W] (7 <= H, W, H*W < 2^31):
+ *   both clamped to [lo, hi] in float32 (NaN stays NaN), then out[5] = {rmse, medae, NaN (the LPIPS slot), ssim, psnr}:
+ *   rmse = sqrt(f32 mean of f32((gt - pred)^2)), medae = np.median(|gt - pred|) exactly, ssim = skimage's
+ *   structural_similarity(pred, gt, data_range = max(gt) - min(gt)) with its constants squared as x*x, and
+ *   psnr = f32(10 log10(f32(peak / mse))) (peak 80^2 for depth, 1 for intensity).  work = l4d_image_metrics_work_bytes(H, W)
+ *   bytes, 16-byte aligned (L4D_ESIZE when smaller); on return it holds the clamped pred at byte offset 0 and the clamped
+ *   gt at byte offset L4D_IM_GT_OFFSET(H, W), each [H, W] fp32.  Four launches.
+ * l4d_raydrop_metrics = RaydropMeter.update on fp32 pred, gt [n] (1 <= n < 2^31): out[3] = {rmse, acc, f1} with
+ *   mask = pred > ratio, acc = count(mask == gt) / n, f1 = 2pr/(p+r) over 64-bit counts (NaN when TP + FP = 0 or
+ *   TP + FN = 0, as in the reference).  One launch. */
+#define L4D_IM_GT_OFFSET(H, W) ((((size_t)(H) * (W) * 4u) + 255u) & ~(size_t)255u)
+size_t l4d_image_metrics_work_bytes(uint32_t H, uint32_t W);
+int    l4d_image_metrics(const float* pred, const float* gt, uint32_t H, uint32_t W, float lo, float hi, float peak,
+                         double* out, void* work, size_t work_bytes, void* stream);
+int    l4d_raydrop_metrics(const float* pred, const float* gt, uint32_t n, float ratio, double* out, void* stream);
+
 /* --- the flow loss's point-cloud preparation (utils/misc.py point_removal, model/runner.py process_pointcloud) ---------
  * Points are row-major [n, 3] float64 unless said otherwise, 1 <= n < 2^31 (else L4D_EINVAL, as for null required
  * pointers).  Compactions keep index order and write their row counts to DEVICE uint32 memory; work buffers of at least

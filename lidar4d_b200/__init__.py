@@ -18,7 +18,8 @@ def __getattr__(name):
     if name in _CONVERT:
         from . import convert
         return getattr(convert, name)
-    if name in ("point_metrics", "PointsMeter"):
+    if name in ("point_metrics", "PointsMeter", "image_metrics", "raydrop_metrics", "DepthMeter", "IntensityMeter",
+                "RaydropMeter"):
         from . import metrics
         return getattr(metrics, name)
     raise AttributeError(name)

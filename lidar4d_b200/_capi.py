@@ -156,6 +156,7 @@ EXPORTS = [
     "l4d_patch_loss", "l4d_patch_loss_backward", "l4d_los_work_bytes", "l4d_los_loss", "l4d_los_loss_backward",
     "l4d_nn_grid_bytes", "l4d_nn_grid_work_bytes", "l4d_nn_grid_build", "l4d_nn_grid_query", "l4d_flow_warp_query",
     "l4d_flow_term_backward", "l4d_flow_ground", "l4d_flow_ground_backward", "l4d_flow_loss_finish",
+    "l4d_image_metrics_work_bytes", "l4d_image_metrics", "l4d_raydrop_metrics",
 ]
 
 
@@ -254,6 +255,12 @@ def declare(lib, prefix: str = "l4d_", host_sim: bool = False):
         lib.l4d_pano_unproject.restype = C.c_int
         lib.l4d_point_metrics.argtypes = [V, U32, V, U32, C.c_float, V, V]
         lib.l4d_point_metrics.restype = C.c_int
+        lib.l4d_image_metrics_work_bytes.argtypes = [U32, U32]
+        lib.l4d_image_metrics_work_bytes.restype = SZ
+        lib.l4d_image_metrics.argtypes = [V, V, U32, U32, C.c_float, C.c_float, C.c_float, V, V, SZ, V]
+        lib.l4d_image_metrics.restype = C.c_int
+        lib.l4d_raydrop_metrics.argtypes = [V, V, U32, C.c_float, V, V]
+        lib.l4d_raydrop_metrics.restype = C.c_int
         D, F = C.c_double, C.c_float
         for n in ("range_filter", "outlier_select", "ground_split"):
             getattr(lib, f"l4d_{n}_work_bytes").argtypes = [U32]

@@ -17,6 +17,7 @@
 #include "l4d_optim.cuh"
 #include "l4d_losses.cuh"
 #include "l4d_nngrid.cuh"
+#include "l4d_imgmetrics.cuh"
 
 // =============================================================================
 // error plumbing
@@ -1788,6 +1789,41 @@ extern "C" int l4d_los_loss_backward(const float* w, const float* z, const float
   int grid = nblk((size_t)n * S);
   if (grid > 8 * sm_count()) grid = 8 * sm_count();
   ++g_launches; k_los_backward<<<grid, 256, 0, (cudaStream_t)stream>>>(w, z, gt, n, S, a, (const L4DLosWork*)work, g_loss, g_w);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+// =============================================================================
+// the depth / intensity / ray-drop evaluation meters (l4d_imgmetrics.cuh)
+// =============================================================================
+extern "C" size_t l4d_image_metrics_work_bytes(uint32_t H, uint32_t W) { return l4d_im_layout(H, W).total; }
+
+extern "C" int l4d_image_metrics(const float* pred, const float* gt, uint32_t H, uint32_t W, float lo, float hi, float peak,
+                                 double* out, void* work, size_t work_bytes, void* stream) {
+  if (!pred || !gt || !out || !work) return l4d_fail(L4D_EINVAL, "l4d_image_metrics: null pointer");
+  if (H < L4D_IM_WIN || W < L4D_IM_WIN || (uint64_t)H * W >= (1ull << 31))
+    return l4d_fail(L4D_EINVAL, "l4d_image_metrics: need 7 <= H, W and H*W < 2^31");
+  if ((uintptr_t)work & 15) return l4d_fail(L4D_EINVAL, "l4d_image_metrics: work must be 16-byte aligned");
+  if (work_bytes < l4d_im_layout(H, W).total) return l4d_fail(L4D_ESIZE, "l4d_image_metrics: work buffer too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  char* wk = (char*)work;
+  ++g_launches; k_im_columns<<<nblk(W, L4D_IM_COL_NT), L4D_IM_COL_NT, 0, st>>>(pred, gt, H, W, lo, hi, wk);
+  L4D_CUDA(cudaGetLastError());
+  ++g_launches; k_im_rows<<<nblk(5 * (size_t)H, L4D_IM_ROW_NT), L4D_IM_ROW_NT, 0, st>>>(H, W, wk);
+  L4D_CUDA(cudaGetLastError());
+  const size_t crop = (size_t)(H - 2 * L4D_IM_R) * (W - 2 * L4D_IM_R);
+  const int parts = nblk(crop, L4D_IM_SSIM_NT) < L4D_IM_PARTS ? nblk(crop, L4D_IM_SSIM_NT) : L4D_IM_PARTS;
+  ++g_launches; k_im_ssim<<<parts, L4D_IM_SSIM_NT, 0, st>>>(H, W, wk);
+  L4D_CUDA(cudaGetLastError());
+  ++g_launches; k_im_finish<<<1, L4D_IM_FIN_NT, 0, st>>>(H, W, (uint32_t)parts, peak, wk, out);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+extern "C" int l4d_raydrop_metrics(const float* pred, const float* gt, uint32_t n, float ratio, double* out, void* stream) {
+  if (!pred || !gt || !out) return l4d_fail(L4D_EINVAL, "l4d_raydrop_metrics: null pointer");
+  if (n == 0 || n >= (1u << 31)) return l4d_fail(L4D_EINVAL, "l4d_raydrop_metrics: need 1 <= n < 2^31");
+  ++g_launches; k_raydrop<<<1, L4D_IM_FIN_NT, 0, (cudaStream_t)stream>>>(pred, gt, n, ratio, out);
   L4D_CUDA(cudaGetLastError());
   return L4D_OK;
 }
