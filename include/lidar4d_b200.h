@@ -449,6 +449,34 @@ int    l4d_ground_split(const double* points, uint32_t n, const uint8_t* mask, d
                         void* work, size_t work_bytes, void* stream);
 int    l4d_pose_transform(const double* points, uint32_t n, double scale, const float* pose, double* out, void* stream);
 
+/* --- LiDAR sweep images (model/simulator.py Simulator.render, model/runner.py Trainer.test / evaluate_one_epoch) --------
+ * l4d_sweep_images: one rendered frame, depth[H*W] and image[H*W, 2] (channel 0 ray drop, channel 1 intensity) float32,
+ *   and optionally the refined ray drop raydrop[H*W] (dtype L4D_SWEEP_F32 or L4D_SWEEP_F16; when NULL, image channel 0
+ *   is the ray drop and dtype must be L4D_SWEEP_F32) -> the 8-bit images the reference writes and the inputs of its
+ *   point cloud.  With r the ray drop, m = r > 0.5 in r's dtype, I the intensity, D the depth:
+ *   L4D_SWEEP_SIM:  panel [3H, W, 3] BGR = {grey u8(r 255), lut_intensity[u8(I m 255)], lut_depth[u8(D m 255)]};
+ *                   pano[H*W] = D m / scale, intensities[H*W] = I m.
+ *   L4D_SWEEP_TEST: with I', D' = I m, D m if test_mask else I, D: panel = [H, W] u8(m 255), then [H, W, 3]
+ *                   lut_intensity[u8(I' 255)], then [H, W, 3] lut_depth[u8(D' 255)]; pano[H*W] = D' / scale.
+ *   L4D_SWEEP_EVAL: panel [6H, W, 3] = {grey u8(r 255), lut_intensity[u8(I 255)], lut_depth[u8(D 255)], grey u8(m 255),
+ *                   lut_intensity[u8(I m 255)], lut_depth[u8(D m 255)]}, the last two products in double.
+ *   r 255 is rounded in r's dtype, everything else in float32 unless said; u8() is NumPy's float -> uint8 cast (truncate,
+ *   low byte of the int32; NaN, inf and values outside the int32 range give 0).  The luts are [256, 3] BGR device tables
+ *   (cv2.applyColorMap of 0..255 with COLORMAP_BONE and COLORMAP_TURBO), required by every layout.  pano is required by
+ *   SIM and TEST, intensities by SIM; the others are ignored.  Panel bytes: L4D_SWEEP_PANEL_BYTES(layout, H, W).
+ *   Null required pointers, H or W = 0, H*W >= 2^31, unknown layout or dtype: L4D_EINVAL.  One launch on `stream`. */
+#define L4D_SWEEP_SIM  0u
+#define L4D_SWEEP_TEST 1u
+#define L4D_SWEEP_EVAL 2u
+#define L4D_SWEEP_F32  0u
+#define L4D_SWEEP_F16  1u
+#define L4D_SWEEP_PANEL_BYTES(layout, H, W) \
+  ((size_t)(H) * (W) * ((layout) == L4D_SWEEP_EVAL ? 18u : (layout) == L4D_SWEEP_TEST ? 7u : 9u))
+int    l4d_sweep_images(const float* depth, const float* image, const void* raydrop_or_null, uint32_t raydrop_dtype,
+                        uint32_t H, uint32_t W, uint32_t layout, float scale, uint32_t test_mask,
+                        const uint8_t* lut_intensity, const uint8_t* lut_depth, uint8_t* panel, float* pano_or_null,
+                        float* intensities_or_null, void* stream);
+
 /* --- profiling aid: while started, CUDA events are recorded on the launch stream around every kernel of
  *     l4d_render_forward / l4d_render_backward.  l4d_profile_stop returns the number of (kernel name, ms)
  *     pairs written (static strings), or a negative error code.  Not thread-safe. --------------------------- */

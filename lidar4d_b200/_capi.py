@@ -157,7 +157,10 @@ EXPORTS = [
     "l4d_nn_grid_bytes", "l4d_nn_grid_work_bytes", "l4d_nn_grid_build", "l4d_nn_grid_query", "l4d_flow_warp_query",
     "l4d_flow_term_backward", "l4d_flow_ground", "l4d_flow_ground_backward", "l4d_flow_loss_finish",
     "l4d_image_metrics_work_bytes", "l4d_image_metrics", "l4d_raydrop_metrics",
+    "l4d_sweep_images",
 ]
+SWEEP_SIM, SWEEP_TEST, SWEEP_EVAL = 0, 1, 2     # L4D_SWEEP_* layouts of l4d_sweep_images
+SWEEP_F32, SWEEP_F16 = 0, 1                     # L4D_SWEEP_* ray-drop dtypes
 
 
 def lib_path() -> str:
@@ -261,6 +264,8 @@ def declare(lib, prefix: str = "l4d_", host_sim: bool = False):
         lib.l4d_image_metrics.restype = C.c_int
         lib.l4d_raydrop_metrics.argtypes = [V, V, U32, C.c_float, V, V]
         lib.l4d_raydrop_metrics.restype = C.c_int
+        lib.l4d_sweep_images.argtypes = [V, V, V, U32, U32, U32, U32, C.c_float, U32, V, V, V, V, V, V]
+        lib.l4d_sweep_images.restype = C.c_int
         D, F = C.c_double, C.c_float
         for n in ("range_filter", "outlier_select", "ground_split"):
             getattr(lib, f"l4d_{n}_work_bytes").argtypes = [U32]

@@ -57,6 +57,14 @@ def lidar_to_pano(local_points, lidar_H, lidar_W, lidar_K, max_depth=80):
 
 
 def _unproject(pano, intensities, lidar_K):
+    out, count = _unproject_device(pano, intensities, lidar_K)
+    # the one device-to-host read: the exact row count (<= H*W < 2^31) is needed to size the result, and it
+    # synchronises with the stream
+    return out[:int(count.item())]
+
+
+def _unproject_device(pano, intensities, lidar_K):
+    """-> (out [H*W, 3 or 4], count [1] int32), both on the device: the first count rows are the cloud.  No host read."""
     lib = _capi.load_library()
     if pano.dim() != 2:
         raise ValueError(f"pano: expected [H, W], got {tuple(pano.shape)}")
@@ -72,9 +80,7 @@ def _unproject(pano, intensities, lidar_K):
                                     fov_up, fov, out.data_ptr(), count.data_ptr(), work.data_ptr(), nwork,
                                     torch.cuda.current_stream(dev).cuda_stream)
     _capi.check(lib, rc, "l4d_pano_unproject")
-    # the one device-to-host read: the exact row count (<= H*W < 2^31) is needed to size the result, and it
-    # synchronises with the stream
-    return out[:int(count.item())]
+    return out, count
 
 
 def pano_to_lidar_with_intensities(pano, intensities, lidar_K):

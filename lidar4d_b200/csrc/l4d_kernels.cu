@@ -18,6 +18,7 @@
 #include "l4d_losses.cuh"
 #include "l4d_nngrid.cuh"
 #include "l4d_imgmetrics.cuh"
+#include "l4d_sweep.cuh"
 
 // =============================================================================
 // error plumbing
@@ -1824,6 +1825,41 @@ extern "C" int l4d_raydrop_metrics(const float* pred, const float* gt, uint32_t 
   if (!pred || !gt || !out) return l4d_fail(L4D_EINVAL, "l4d_raydrop_metrics: null pointer");
   if (n == 0 || n >= (1u << 31)) return l4d_fail(L4D_EINVAL, "l4d_raydrop_metrics: need 1 <= n < 2^31");
   ++g_launches; k_raydrop<<<1, L4D_IM_FIN_NT, 0, (cudaStream_t)stream>>>(pred, gt, n, ratio, out);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+// =============================================================================
+// LiDAR sweep images of the simulator, Trainer.test and the validation panel (l4d_sweep.cuh)
+// =============================================================================
+extern "C" int l4d_sweep_images(const float* depth, const float* image, const void* raydrop, uint32_t raydrop_dtype,
+                                uint32_t H, uint32_t W, uint32_t layout, float scale, uint32_t test_mask,
+                                const uint8_t* lut_intensity, const uint8_t* lut_depth, uint8_t* panel, float* pano,
+                                float* intensities, void* stream) {
+  if (layout > L4D_SWEEP_EVAL) return l4d_fail(L4D_EINVAL, "l4d_sweep_images: unknown layout");
+  if (raydrop_dtype > L4D_SWEEP_F16 || (!raydrop && raydrop_dtype != L4D_SWEEP_F32))
+    return l4d_fail(L4D_EINVAL, "l4d_sweep_images: unknown ray-drop dtype (or float16 without a ray-drop map)");
+  if (!depth || !image || !panel) return l4d_fail(L4D_EINVAL, "l4d_sweep_images: null pointer");
+  if (!lut_intensity || !lut_depth) return l4d_fail(L4D_EINVAL, "l4d_sweep_images: null colour table");
+  if (layout != L4D_SWEEP_EVAL && !pano) return l4d_fail(L4D_EINVAL, "l4d_sweep_images: null pano");
+  if (layout == L4D_SWEEP_SIM && !intensities) return l4d_fail(L4D_EINVAL, "l4d_sweep_images: null intensities");
+  if (H == 0 || W == 0 || (uint64_t)H * W >= (1ull << 31))
+    return l4d_fail(L4D_EINVAL, "l4d_sweep_images: need 1 <= H, W and H*W < 2^31");
+  L4DSweepArgs A;
+  A.depth = depth;
+  A.image = image;
+  A.raydrop = raydrop;
+  A.lut[0] = lut_intensity;
+  A.lut[1] = lut_depth;
+  A.panel = panel;
+  A.pano = pano;
+  A.inten = intensities;
+  A.hw = H * W;
+  A.layout = layout;
+  A.is_f16 = raydrop && raydrop_dtype == L4D_SWEEP_F16;
+  A.test_mask = test_mask != 0;
+  A.scale = scale;
+  ++g_launches; k_sweep_images<<<nblk(A.hw, L4D_SWEEP_NT), L4D_SWEEP_NT, 0, (cudaStream_t)stream>>>(A);
   L4D_CUDA(cudaGetLastError());
   return L4D_OK;
 }
