@@ -202,53 +202,15 @@ L4D_WARP_FN WarpRuns l4d_warp_runs(int key) {
 }
 // inclusive segmented scans of 8 values at once (8 independent shuffles per step); the tail lane of a run ends up
 // with the run's sums
-#ifndef L4D_SCAN_FMA
-#define L4D_SCAN_FMA 1
-#endif
 L4D_WARP_FN void l4d_seg_sum8(float (&v)[8], const WarpRuns& r) {
   // only as many steps as the longest run of the warp needs (measured against a fixed 5-step scan: 14.2 -> 11.8 ms)
 #pragma unroll 1
   for (int d = 1; d <= r.maxdist; d <<= 1) {
-#if L4D_SCAN_FMA
     // one FFMA per value instead of FSEL + FADD (the scans are 40 % of this kernel's instructions): fma(t, 1, v) rounds
     // like t + v, fma(t, 0, v) = v for every finite t
     const float take = r.dist >= d ? 1.0f : 0.0f;
 #pragma unroll
     for (int c = 0; c < 8; ++c) v[c] = fmaf(__shfl_up_sync(0xffffffffu, v[c], d), take, v[c]);
-#else
-    const bool take = r.dist >= d;
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      const float t = __shfl_up_sync(0xffffffffu, v[c], d);
-      v[c] += take ? t : 0.f;
-    }
-#endif
-  }
-}
-// (A/B option, measured 3.5x SLOWER than the scans - REDUX with per-run member masks is far from one result per clock -
-// kept for the record, off by default.)
-// Run sums with ONE warp reduction per value instead of a log-depth scan: every run agrees on a power-of-two scale from
-// its largest magnitude (redux.max on the float bit patterns), the values go to 32-bit fixed point (|v| < 2^25, so 32 of
-// them cannot overflow), redux.sync.add over the run's lanes sums them exactly and order-independently, and the result is
-// scaled back.  Quantisation: 2^-25 of the run's largest term per addend - below fp32 summation noise of the same sum.
-// Every lane of the run receives the sums; straight-line code, so runs of one warp do not diverge.
-#ifndef L4D_RUNSUM_REDUX
-#define L4D_RUNSUM_REDUX 0
-#endif
-template <int N>
-L4D_WARP_FN void l4d_run_sum(float (&v)[N], const WarpRuns& r) {
-  if (r.maxdist == 0) return;                       // warp-uniform: every lane is its own run
-  float am = 0.f;
-#pragma unroll
-  for (int i = 0; i < N; ++i) am = fmaxf(am, fabsf(v[i]));
-  const unsigned amb = __reduce_max_sync(r.mask, __float_as_uint(am));      // non-negative floats order like their bits
-  int e = (int)(amb >> 23) - 127;                   // run amax in [2^e, 2^(e+1))
-  e = e < -100 ? -100 : (e > 100 ? 100 : e);        // keep 2^(24-e) and 2^(e-24) normal (|gradients| beyond 2^+-100 do not occur)
-  const float sc = __uint_as_float((unsigned)(127 + 24 - e) << 23), inv = __uint_as_float((unsigned)(127 - 24 + e) << 23);
-#pragma unroll
-  for (int i = 0; i < N; ++i) {
-    const int q = __reduce_add_sync(r.mask, __float2int_rn(v[i] * sc));
-    v[i] = (float)q * inv;
   }
 }
 // all 32 lanes must call; g may be zero for lanes without a contribution
@@ -262,11 +224,7 @@ L4D_WARP_FN void l4d_plane_scatter_warp(float* G, int W, const Bilerp& b, const 
     float s[8];
 #pragma unroll
     for (int c = 0; c < 8; ++c) s[c] = g[c] * wgt[k];
-#if L4D_RUNSUM_REDUX
-    l4d_run_sum<8>(s, r);
-#else
     l4d_seg_sum8(s, r);
-#endif
     if (r.tail) {
       float* p = G + ((size_t)ys[k] * W + xs[k]) * 8;
       l4d_red4(p, s[0], s[1], s[2], s[3]);
@@ -280,13 +238,8 @@ L4D_WARP_FN void l4d_plane_scatter_warp_t(float* G, int W, const Bilerp& b, cons
   float s0[8], s1[8];
 #pragma unroll
   for (int c = 0; c < 8; ++c) { s0[c] = g[c] * b.wx0; s1[c] = g[c] * b.wx1; }
-#if L4D_RUNSUM_REDUX
-  l4d_run_sum<8>(s0, r);
-  l4d_run_sum<8>(s1, r);
-#else
   l4d_seg_sum8(s0, r);
   l4d_seg_sum8(s1, r);
-#endif
   if (r.tail) {
     float* p00 = G + ((size_t)b.y0 * W + b.x0) * 8;
     float* p01 = G + ((size_t)b.y0 * W + b.x1) * 8;
@@ -311,13 +264,8 @@ L4D_WARP_FN void l4d_row_scatter_warp(float* Grow, const Bilerp& b, const float 
   float s0[8], s1[8];
 #pragma unroll
   for (int c = 0; c < 8; ++c) { s0[c] = g[c] * b.wx0; s1[c] = g[c] * b.wx1; }
-#if L4D_RUNSUM_REDUX
-  l4d_run_sum<8>(s0, r);
-  l4d_run_sum<8>(s1, r);
-#else
   l4d_seg_sum8(s0, r);
   l4d_seg_sum8(s1, r);
-#endif
   if (r.tail) {
     float* p0 = Grow + (size_t)b.x0 * 8;
     float* p1 = Grow + (size_t)b.x1 * 8;
@@ -505,20 +453,6 @@ struct DfeatFromPlane {
   L4D_HD void ld4(int row, float (&o)[4]) const { for (int i = 0; i < 4; ++i) o[i] = (*this)(row + i); }
 };
 
-// scatter dL/dfeature through the encoders of one sample at (x,y,z) with its flow; dflow[6] out
-// PARTS: which sinks this instantiation serves (the split pipeline runs them as separate kernels so that each keeps
-// fewer values live: bit 0 static planes, bit 1 time planes (+ dL/dflow), bit 2 dynamic hash)
-#define L4D_SC_STATIC_PLANES 1
-#define L4D_SC_TIME_PLANES 2
-#define L4D_SC_DYNAMIC_HASH 4
-#define L4D_SC_ALL 7
-// L4D_SCATTER_INTERLEAVE (A/B knob, default off): issue the dynamic-hash REDs in slices BETWEEN the plane sinks instead of back to
-// back at the end (1 = one slice per time-plane query, 2 = one per plane sink).  The idea - the sinks are issue / shuffle work,
-// the REDs L2-atomic work, let them overlap inside a warp - not measured on the H100; off because the warps of an SM already
-// sit in different phases.
-#ifndef L4D_SCATTER_INTERLEAVE
-#define L4D_SCATTER_INTERLEAVE 0
-#endif
 struct DynHashCursor {
   int p, l;            // next (plane, level)
   float dq[4];         // dL/dfeature of levels (l & ~3) .. +3 of plane p (valid when the level count is a multiple of 4)
@@ -604,7 +538,8 @@ L4D_HD void l4d_bw_dynhash_slice(const DevModel& M, const L4DFrame& F, const Dev
   }
 }
 
-template <bool WARP_AGG, class DF, bool STATIC_HASH = true, int PARTS = L4D_SC_ALL, bool ROWS = false>
+// scatter dL/dfeature through the encoders of one sample at (x,y,z) with its flow; dflow[6] out
+template <bool WARP_AGG, class DF, bool STATIC_HASH = true, bool ROWS = false>
 L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrads& G, float x, float y, float z,
                              const float* flow, const DF& l4d_dfeat_fn, float (&dflow)[6], bool active, int seg = 0);
 
@@ -614,13 +549,13 @@ L4D_HD void l4d_bw_scatter(const DevModel& M, const L4DFrame& F, const DevGrads&
   for (int k = 0; k < 6; ++k) s.dflow[k] = 0.f;
   if (!s.active) return;
   DfeatFromDh df{&M, &s};
-  l4d_bw_scatter_t<false, DfeatFromDh, true, L4D_SC_ALL, ROWS>(M, F, G, s.x, s.y, s.z, s.flow, df, s.dflow, true);
+  l4d_bw_scatter_t<false, DfeatFromDh, true, ROWS>(M, F, G, s.x, s.y, s.z, s.flow, df, s.dflow, true);
 }
 
 // ROWS: time planes are sampled from DevModel::pl_con and their gradients go to DevGrads::pl_rows (both must be set)
 // WARP_AGG: every lane of the warp must call (lanes without a sample pass active=false and a
 // provider that returns 0; they take part in the plane aggregation with zero contributions); seg: the sample's ray
-template <bool WARP_AGG, class DF, bool STATIC_HASH, int PARTS, bool ROWS>
+template <bool WARP_AGG, class DF, bool STATIC_HASH, bool ROWS>
 L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrads& G, float x, float y, float z,
                              const float* flow, const DF& l4d_dfeat_fn, float (&dflow)[6], bool active, int seg) {
 #pragma unroll
@@ -634,21 +569,16 @@ L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrad
   l4d_agg_weights(F, wc, wf, wb);
   const float xf0 = x + flow[0], xf1 = y + flow[1], xf2 = z + flow[2];
   const float xw0 = x + flow[3], xw1 = y + flow[4], xw2 = z + flow[5];
-  // dynamic-hash REDs are spread over the plane work (see L4D_SCATTER_INTERLEAVE above)
   DynHashCursor hc;
-  hc.p = (PARTS & L4D_SC_DYNAMIC_HASH) ? 0 : 3;
+  hc.p = 0;
   hc.l = 0;
   hc.dq[0] = hc.dq[1] = hc.dq[2] = hc.dq[3] = 0.f;
-  const int hslots = L4D_SCATTER_INTERLEAVE == 2 ? nS * 12 : nS * 3;
-  const int hper = L4D_SCATTER_INTERLEAVE ? (3 * L + hslots - 1) / hslots : 0;
-#define L4D_DYNHASH_SLICE(mode, n) \
-  do { if (L4D_SCATTER_INTERLEAVE == (mode)) l4d_bw_dynhash_slice<WARP_AGG>(M, F, G, x, y, z, wc, l4d_dfeat_fn, row_hash_d, hc, (n), seg, active); } while (0)
 
 #pragma unroll 1
   for (int sc = 0; sc < nS; ++sc) {
     const int R = (int)M.plane_res[sc];
     const int T = (int)M.time_res;
-    if (PARTS & L4D_SC_STATIC_PLANES) {   // static planes: product rule over (x,y) (x,z) (y,z)
+    {   // static planes: product rule over (x,y) (x,z) (y,z)
       float d[8], v0[8], v1[8], v2[8], dummy[8], g[8];
 #pragma unroll
       for (int c = 0; c < 8; c += 4) l4d_dfeat_fn.ld4(sc * 8 + c, *reinterpret_cast<float(*)[4]>(d + c));
@@ -659,17 +589,14 @@ L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrad
 #pragma unroll
       for (int c = 0; c < 8; ++c) g[c] = d[c] * v1[c] * v2[c];
       l4d_plane_sink<WARP_AGG>(G.planes_cl[sc][0], R, b0, g, false);
-      L4D_DYNHASH_SLICE(2, hper);
 #pragma unroll
       for (int c = 0; c < 8; ++c) g[c] = d[c] * v0[c] * v2[c];
       l4d_plane_sink<WARP_AGG>(G.planes_cl[sc][1], R, b1, g, false);
-      L4D_DYNHASH_SLICE(2, hper);
 #pragma unroll
       for (int c = 0; c < 8; ++c) g[c] = d[c] * v0[c] * v1[c];
       l4d_plane_sink<WARP_AGG>(G.planes_cl[sc][3], R, b2, g, false);
-      L4D_DYNHASH_SLICE(2, hper);
     }
-    if (PARTS & L4D_SC_TIME_PLANES) {   // time planes (x,t) (y,t) (z,t): three queries, warped ones also feed d(coords) -> flow
+    {   // time planes (x,t) (y,t) (z,t): three queries, warped ones also feed d(coords) -> flow
       float d[8];
 #pragma unroll
       for (int c = 0; c < 8; c += 4) l4d_dfeat_fn.ld4(row_plane_d + sc * 8 + c, *reinterpret_cast<float(*)[4]>(d + c));
@@ -698,18 +625,14 @@ L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrad
 #pragma unroll
         for (int c = 0; c < 8; ++c) { g[c] = wq * d[c] * v1[c] * v2[c]; c0 = fmaf(g[c], x0[c], c0); }
         if (rows) l4d_row_sink<WARP_AGG>(G.pl_rows[sc][0][qi], b0, g); else l4d_plane_sink<WARP_AGG>(G.planes_cl[sc][2], R, b0, g, true);
-        L4D_DYNHASH_SLICE(2, hper);
 #pragma unroll
         for (int c = 0; c < 8; ++c) { g[c] = wq * d[c] * v0[c] * v2[c]; c1 = fmaf(g[c], x1[c], c1); }
         if (rows) l4d_row_sink<WARP_AGG>(G.pl_rows[sc][1][qi], b1, g); else l4d_plane_sink<WARP_AGG>(G.planes_cl[sc][4], R, b1, g, true);
-        L4D_DYNHASH_SLICE(2, hper);
 #pragma unroll
         for (int c = 0; c < 8; ++c) { g[c] = wq * d[c] * v0[c] * v1[c]; c2 = fmaf(g[c], x2[c], c2); }
         if (rows) l4d_row_sink<WARP_AGG>(G.pl_rows[sc][2][qi], b2, g); else l4d_plane_sink<WARP_AGG>(G.planes_cl[sc][5], R, b2, g, true);
-        L4D_DYNHASH_SLICE(2, hper);
         if (qi == 1) { dflow[0] += c0; dflow[1] += c1; dflow[2] += c2; }
         if (qi == 2) { dflow[3] += c0; dflow[4] += c1; dflow[5] += c2; }
-        L4D_DYNHASH_SLICE(1, hper);
       }
     }
   }
@@ -728,9 +651,8 @@ L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrad
     for (int c = 0; c < 8; ++c) l4d_red4(base + (size_t)idx[c] * 4, w[c] * d0, w[c] * d1, w[c] * d2, w[c] * d3);
   }
 
-  // dynamic hash: whatever the slices above did not cover (all of it when L4D_SCATTER_INTERLEAVE == 0)
+  // dynamic hash
   l4d_bw_dynhash_slice<WARP_AGG>(M, F, G, x, y, z, wc, l4d_dfeat_fn, row_hash_d, hc, 3 * L, seg, active);
-#undef L4D_DYNHASH_SLICE
 }
 
 // ---- B5: flow MLP backprop.  g[6] = dL/dflow of this sample. ----------------------------

@@ -357,43 +357,14 @@ L4D_HD float l4d_contract_entry(uint4 rec, const L4DTimeQuery& q, uint32_t n_sli
   }
   return ((q.basis[0] * fl[0] + q.basis[1] * fl[1]) + q.basis[2] * fl[2]) + q.basis[3] * fl[3];
 }
-// one level of one contracted dynamic table at (x,y): bilinear blend of four fp32 entries.
-// L4D_CON_GATHER (A/B knob; timings not measured on the H100):
-//   0  one 16-byte load of the aligned quad of entries that holds the first x-corner (the second x-corner is in the same
-//      quad three times out of four) + a conditional 4-byte load otherwise: fewer sector requests per level, but a
-//      divergent branch per row, so the loads of a level no longer overlap
-//   1  four independent 4-byte loads (no branch, no selects): the default
-//   2  the quad load + an unconditional 4-byte load of the second x-corner
-#ifndef L4D_CON_GATHER
-#define L4D_CON_GATHER 1
-#endif
+// one level of one contracted dynamic table at (x,y): bilinear blend of four fp32 entries, as four independent 4-byte
+// loads (what the gather is short of is requests in flight, not sectors: DESIGN.md 9)
 L4D_HD float l4d_encode2_con(const DevGrid& g, const float* con, int l, float x, float y) {
   uint32_t idx[4]; float w[4];
   l4d_corners2(g, l, x, y, idx, w);
-  const float* base = con + g.offset[l];          // level offsets are multiples of 8 entries: quads are 16-byte aligned
-#if L4D_CON_GATHER == 1
+  const float* base = con + g.offset[l];
   const float v0 = l4d_ld1(base + idx[0]), v1 = l4d_ld1(base + idx[1]), v2 = l4d_ld1(base + idx[2]), v3 = l4d_ld1(base + idx[3]);
   return fmaf(w[3], v3, fmaf(w[2], v2, fmaf(w[1], v1, w[0] * v0)));
-#else
-  float out = 0.f;
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const uint32_t i0 = idx[2 * r], i1 = idx[2 * r + 1];
-    const float4 q = l4d_ld4(base + (i0 & ~3u));
-    const uint32_t s0 = i0 & 3u;
-    const float v0 = s0 == 0u ? q.x : (s0 == 1u ? q.y : (s0 == 2u ? q.z : q.w));
-#if L4D_CON_GATHER == 2
-    const float v1 = l4d_ld1(base + i1);
-#else
-    const uint32_t s1 = i1 & 3u;
-    float v1 = s1 == 0u ? q.x : (s1 == 1u ? q.y : (s1 == 2u ? q.z : q.w));
-    if ((i0 >> 2) != (i1 >> 2)) v1 = l4d_ld1(base + i1);
-#endif
-    out = fmaf(w[2 * r], v0, out);
-    out = fmaf(w[2 * r + 1], v1, out);
-  }
-  return out;
-#endif
 }
 
 // ---------------------------------------------------------------------------

@@ -265,17 +265,17 @@ static inline DensitySavedLayout density_saved_layout(const L4DConfig* c, uint32
   return L;
 }
 
-// DevModel::hd_con inside the saved buffer of a launch (level offsets, hence plane sizes, are multiples of 8 entries)
-// mode bit 0: dynamic-hash tables, bit 1: time-plane rows
-static inline void point_contracted(const L4DConfig* c, void* saved, uint32_t n_rays, uint32_t S, DevModel& M, int mode) {
+// DevModel::hd_con (dynamic-hash tables) and ::pl_con (time-plane rows) inside the saved buffer of a launch (level offsets,
+// hence plane sizes, are multiples of 8 entries)
+static inline void point_contracted(const L4DConfig* c, void* saved, uint32_t n_rays, uint32_t S, DevModel& M) {
   SavedLayout L = saved_layout(c, n_rays, S);
   float* b = reinterpret_cast<float*>(reinterpret_cast<char*>(saved) + L.hd_con);
-  for (int q = 0; (mode & 1) && q < 3; ++q)
+  for (int q = 0; q < 3; ++q)
     for (int p = 0; p < 3; ++p) {
       M.hd_con[p][q] = b;
       b += c->hash_dynamic[p].offset[c->hash_dynamic[p].n_levels];
     }
-  if (mode & 2) point_time_rows<const float>(c, reinterpret_cast<const float*>(reinterpret_cast<char*>(saved) + L.pl_con), M.pl_con);
+  point_time_rows<const float>(c, reinterpret_cast<const float*>(reinterpret_cast<char*>(saved) + L.pl_con), M.pl_con);
 }
 static inline SavedView saved_view(const L4DConfig* c, void* saved, uint32_t n_rays, uint32_t S) {
   SavedLayout L = saved_layout(c, n_rays, S);

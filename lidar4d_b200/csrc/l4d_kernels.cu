@@ -1102,8 +1102,7 @@ static int grid_for(K kernel, int nt, size_t smem, uint32_t work, int& grid, int
       else if (n_set < 32) smem_set[n_set++] = SmemSet{key, smem};
     }
   }
-  static const bool no_memo = getenv("L4D_NO_MEMO") != nullptr;      // developer A/B knob
-  for (int i = 0; i < n_memo && !no_memo; ++i)
+  for (int i = 0; i < n_memo; ++i)
     if (memo[i].k == key && memo[i].smem == smem && memo[i].nt == nt && memo[i].force == force_per_sm) { per_sm = memo[i].per_sm; break; }
   if (per_sm == 0) {
     cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, nt, smem);
@@ -1118,7 +1117,7 @@ static int grid_for(K kernel, int nt, size_t smem, uint32_t work, int& grid, int
       if (pct > 100) pct = 100;
       cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
     }
-    if (n_memo < 64 && !no_memo) memo[n_memo++] = Memo{key, smem, nt, force_per_sm, per_sm};
+    if (n_memo < 64) memo[n_memo++] = Memo{key, smem, nt, force_per_sm, per_sm};
   }
   long g = (long)per_sm * sm_count();
   if ((long)work < g) g = work;
@@ -1127,14 +1126,6 @@ static int grid_for(K kernel, int nt, size_t smem, uint32_t work, int& grid, int
   return L4D_OK;
 }
 
-// Per-launch contraction of the time-dependent encoders with the frame's constants (split pipeline).  L4D_CONTRACT is an
-// A/B knob: bit 0 = dynamic-hash tables (DevModel::hd_con), bit 1 = time-plane rows (DevModel::pl_con, DevGrads::pl_rows);
-// 0 = gather / scatter on the parameters' own layouts as in round 1.
-static int contract_mode() {
-  static const char* e = getenv("L4D_CONTRACT");
-  static const int m = e ? atoi(e) & 3 : 3;
-  return m;
-}
 static void fill_split(SplitArgs& A, const L4DConfig* cfg, const void* staged, const L4DFrame* frame, const L4DRays* rays,
                        void* saved) {
   memset(&A, 0, sizeof(A));
@@ -1200,39 +1191,38 @@ extern "C" int l4d_render_forward(const L4DConfig* cfg, const void* staged, cons
   A.depth = depth; A.image = image; A.wsum = wsum; A.weights = weights; A.zvals = zvals;
   A.train = 1u;
   const size_t P = (size_t)rays->n_rays * rays->n_steps;
-  const int cmode = contract_mode();
-  point_contracted(cfg, saved, rays->n_rays, rays->n_steps, A.M, cmode);
+  // per-launch contraction of the time-dependent encoders with the frame's constants: dynamic-hash tables
+  // (DevModel::hd_con) and time-plane rows (DevModel::pl_con)
+  point_contracted(cfg, saved, rays->n_rays, rays->n_steps, A.M);
   {
-    if (cmode & 1) {
-      ContractArgs C;
-      memset(&C, 0, sizeof(C));
-      uint32_t nmax = 0;
-      for (int p = 0; p < 3; ++p) {
-        C.table[p] = reinterpret_cast<const uint4*>(A.M.hd[p]);
-        C.entries[p] = A.M.hd_slice_entries[p];
-        nmax = C.entries[p] > nmax ? C.entries[p] : nmax;
-        for (int q = 0; q < 3; ++q) C.con[p][q] = const_cast<float*>(A.M.hd_con[p][q]);
-      }
-      C.n_slices = cfg->time_resolution;
-      C.n_queries_mask = 1u | (frame->has_fwd ? 2u : 0u) | (frame->has_bwd ? 4u : 0u);
-      C.q[0] = frame->cur; C.q[1] = frame->fwd; C.q[2] = frame->bwd;
-      ++g_launches; k_contract_dynamic<<<dim3((unsigned)nblk(nmax), 3), 256, 0, st>>>(C);
+    ContractArgs C;
+    memset(&C, 0, sizeof(C));
+    uint32_t nmax = 0;
+    for (int p = 0; p < 3; ++p) {
+      C.table[p] = reinterpret_cast<const uint4*>(A.M.hd[p]);
+      C.entries[p] = A.M.hd_slice_entries[p];
+      nmax = C.entries[p] > nmax ? C.entries[p] : nmax;
+      for (int q = 0; q < 3; ++q) C.con[p][q] = const_cast<float*>(A.M.hd_con[p][q]);
     }
-    if (cmode & 2) {
-      TimeRowArgs T;
-      fill_time_rows(T, cfg, frame);
-      uint32_t rmax = 0;
-      for (uint32_t s2 = 0; s2 < cfg->n_plane_scales; ++s2) {
-        rmax = cfg->plane_res[s2] > rmax ? cfg->plane_res[s2] : rmax;
-        for (int t = 0; t < 3; ++t) {
-          T.plane[s2][t] = const_cast<float*>(A.M.planes[s2][t == 0 ? 2 : (t == 1 ? 4 : 5)]);
-          for (int q = 0; q < 3; ++q) T.row[s2][t][q] = const_cast<float*>(A.M.pl_con[s2][t][q]);
-        }
-      }
-      ++g_launches; k_contract_planes<<<dim3((unsigned)nblk((size_t)rmax * 8), 3 * cfg->n_plane_scales), 256, 0, st>>>(T);
-    }
-    if (cmode) prof_mark(st, "k_contract");
+    C.n_slices = cfg->time_resolution;
+    C.n_queries_mask = 1u | (frame->has_fwd ? 2u : 0u) | (frame->has_bwd ? 4u : 0u);
+    C.q[0] = frame->cur; C.q[1] = frame->fwd; C.q[2] = frame->bwd;
+    ++g_launches; k_contract_dynamic<<<dim3((unsigned)nblk(nmax), 3), 256, 0, st>>>(C);
   }
+  {
+    TimeRowArgs T;
+    fill_time_rows(T, cfg, frame);
+    uint32_t rmax = 0;
+    for (uint32_t s2 = 0; s2 < cfg->n_plane_scales; ++s2) {
+      rmax = cfg->plane_res[s2] > rmax ? cfg->plane_res[s2] : rmax;
+      for (int t = 0; t < 3; ++t) {
+        T.plane[s2][t] = const_cast<float*>(A.M.planes[s2][t == 0 ? 2 : (t == 1 ? 4 : 5)]);
+        for (int q = 0; q < 3; ++q) T.row[s2][t][q] = const_cast<float*>(A.M.pl_con[s2][t][q]);
+      }
+    }
+    ++g_launches; k_contract_planes<<<dim3((unsigned)nblk((size_t)rmax * 8), 3 * cfg->n_plane_scales), 256, 0, st>>>(T);
+  }
+  prof_mark(st, "k_contract");
   if (cfg->mlp_fp16) {
     {
       const size_t smem = tc_dyn_smem(flow_tc_smem().total_fwd);
@@ -1315,8 +1305,7 @@ extern "C" int l4d_render_backward_ex(const L4DConfig* cfg, const void* staged, 
     SplitArgs A;
     fill_split(A, cfg, staged, frame, rays, const_cast<void*>(saved));
     build_grads(cfg, grads, grad_work, A.G, true);
-    const bool rows = (contract_mode() & 2) != 0;        // the forward of this launch left the contracted time planes in `saved`
-    if (rows) point_contracted(cfg, const_cast<void*>(saved), rays->n_rays, rays->n_steps, A.M, 2);
+    point_contracted(cfg, const_cast<void*>(saved), rays->n_rays, rays->n_steps, A.M);   // what the forward left in `saved`
     A.g_depth = g_depth; A.g_image = g_image; A.g_wsum = g_wsum; A.g_weights = g_weights;
     A.train = 1u;
     const size_t P = (size_t)rays->n_rays * rays->n_steps;
@@ -1339,46 +1328,22 @@ extern "C" int l4d_render_backward_ex(const L4DConfig* cfg, const void* staged, 
     }
     {
       int grid;
-      {
-        // default: ONE kernel (its dynamic-hash reductions drain under the plane arithmetic).  L4D_SCATTER_SPLIT=1 (A/B knob)
-        // runs the time planes and the static planes + dynamic hash as two kernels at higher occupancy: measured slower,
-        // 17.1 + 12.7 ms vs 26.6 ms per 16,384 rays (DESIGN.md 9)
-        static const char* e = getenv("L4D_SCATTER_SPLIT");
-        const bool split = e && atoi(e) != 0;
-        if (split) {
-          rc = grid_for(k_bwd_scatter<L4D_NT, L4D_SC_TIME_PLANES, L4D_SCATTER_T_CTAS>, L4D_NT, 0, tiles, grid);
-          if (rc != L4D_OK) return rc;
-          ++g_launches; k_bwd_scatter<L4D_NT, L4D_SC_TIME_PLANES, L4D_SCATTER_T_CTAS><<<grid, L4D_NT, 0, st>>>(A);
-          prof_mark(st, "k_bwd_scatter_time");
-          rc = grid_for(k_bwd_scatter<L4D_NT, L4D_SC_STATIC_PLANES | L4D_SC_DYNAMIC_HASH, L4D_SCATTER_S_CTAS>, L4D_NT, 0, tiles, grid);
-          if (rc != L4D_OK) return rc;
-          ++g_launches; k_bwd_scatter<L4D_NT, L4D_SC_STATIC_PLANES | L4D_SC_DYNAMIC_HASH, L4D_SCATTER_S_CTAS><<<grid, L4D_NT, 0, st>>>(A);
-          prof_mark(st, "k_bwd_scatter_sd");
-        } else {
-          if (rows) {
-            rc = grid_for(k_bwd_scatter<L4D_NT, L4D_SC_ALL, L4D_SCATTER_MIN_CTAS, true>, L4D_NT, 0, tiles, grid);
-            if (rc != L4D_OK) return rc;
-            ++g_launches; k_bwd_scatter<L4D_NT, L4D_SC_ALL, L4D_SCATTER_MIN_CTAS, true><<<grid, L4D_NT, 0, st>>>(A);
-          } else {
-            rc = grid_for(k_bwd_scatter<L4D_NT, L4D_SC_ALL, L4D_SCATTER_MIN_CTAS>, L4D_NT, 0, tiles, grid);
-            if (rc != L4D_OK) return rc;
-            ++g_launches; k_bwd_scatter<L4D_NT, L4D_SC_ALL, L4D_SCATTER_MIN_CTAS><<<grid, L4D_NT, 0, st>>>(A);
+      rc = grid_for(k_bwd_scatter<L4D_NT, L4D_SCATTER_MIN_CTAS>, L4D_NT, 0, tiles, grid);
+      if (rc != L4D_OK) return rc;
+      ++g_launches; k_bwd_scatter<L4D_NT, L4D_SCATTER_MIN_CTAS><<<grid, L4D_NT, 0, st>>>(A);
+      prof_mark(st, "k_bwd_scatter");
+      {       // gradient rows -> the two live time rows of every time plane
+        TimeRowArgs T;
+        fill_time_rows(T, cfg, frame);
+        uint32_t rmax = 0;
+        for (uint32_t s2 = 0; s2 < cfg->n_plane_scales; ++s2) {
+          rmax = cfg->plane_res[s2] > rmax ? cfg->plane_res[s2] : rmax;
+          for (int t = 0; t < 3; ++t) {
+            T.plane[s2][t] = A.G.planes_cl[s2][t == 0 ? 2 : (t == 1 ? 4 : 5)];
+            for (int q = 0; q < 3; ++q) T.row[s2][t][q] = A.G.pl_rows[s2][t][q];
           }
-          prof_mark(st, "k_bwd_scatter");
         }
-        if (rows && !split) {       // gradient rows -> the two live time rows of every time plane
-          TimeRowArgs T;
-          fill_time_rows(T, cfg, frame);
-          uint32_t rmax = 0;
-          for (uint32_t s2 = 0; s2 < cfg->n_plane_scales; ++s2) {
-            rmax = cfg->plane_res[s2] > rmax ? cfg->plane_res[s2] : rmax;
-            for (int t = 0; t < 3; ++t) {
-              T.plane[s2][t] = A.G.planes_cl[s2][t == 0 ? 2 : (t == 1 ? 4 : 5)];
-              for (int q = 0; q < 3; ++q) T.row[s2][t][q] = A.G.pl_rows[s2][t][q];
-            }
-          }
-          ++g_launches; k_fold_planes<<<dim3((unsigned)nblk((size_t)rmax * 8), 3 * cfg->n_plane_scales), 256, 0, st>>>(T);
-        }
+        ++g_launches; k_fold_planes<<<dim3((unsigned)nblk((size_t)rmax * 8), 3 * cfg->n_plane_scales), 256, 0, st>>>(T);
       }
       rc = grid_for(k_bwd_scatter_static<L4D_NT>, L4D_NT, 0, tiles, grid);
       if (rc != L4D_OK) return rc;

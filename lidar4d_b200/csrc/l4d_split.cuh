@@ -349,12 +349,6 @@ __global__ void __launch_bounds__(NT) k_bwd_dense(const __grid_constant__ SplitA
 #ifndef L4D_SCATTER_MIN_CTAS
 #define L4D_SCATTER_MIN_CTAS 4
 #endif
-#ifndef L4D_SCATTER_T_CTAS       // time-plane kernel
-#define L4D_SCATTER_T_CTAS 3
-#endif
-#ifndef L4D_SCATTER_S_CTAS       // static-plane + dynamic-hash kernel
-#define L4D_SCATTER_S_CTAS 4
-#endif
 struct DfeatFromTile {
   const float* base;     // this sample's row in its dfeat tile
   bool on;
@@ -365,9 +359,8 @@ struct DfeatFromTile {
   }
 };
 
-// PARTS selects the sinks (l4d_bwd.cuh).  Default = all of them in one kernel; the two-kernel variant (time planes, which
-// need the flow and produce dL/dflow | static planes + dynamic hash at 4 CTAs/SM) is an A/B option that measured slower.
-template <int NT, int PARTS, int MIN_CTAS, bool ROWS = false>
+// the time planes come from the forward's contracted rows (DevModel::pl_con) and reduce into DevGrads::pl_rows
+template <int NT, int MIN_CTAS>
 __global__ void __launch_bounds__(NT, MIN_CTAS) k_bwd_scatter(const __grid_constant__ SplitArgs A) {
   const DevModel& M = A.M;
   const size_t P = A.sv.P;
@@ -385,10 +378,10 @@ __global__ void __launch_bounds__(NT, MIN_CTAS) k_bwd_scatter(const __grid_const
     const float z = l4d_x01(__ldg(A.rays_o + 3 * ray + 2), __ldg(A.rays_d + 3 * ray + 2), zj, M.bound);
     float flow[6], dflow[6];
 #pragma unroll
-    for (int k = 0; k < 6; ++k) flow[k] = (PARTS & L4D_SC_TIME_PLANES) ? A.sv.flow[(size_t)k * P + p] : 0.f;
+    for (int k = 0; k < 6; ++k) flow[k] = A.sv.flow[(size_t)k * P + p];
     DfeatFromTile df{A.sv.dfeat + l4d_dfeat_off(A.sv, ray, j), active};
-    l4d_bw_scatter_t<true, DfeatFromTile, false, PARTS, ROWS>(M, A.F, A.G, x, y, z, flow, df, dflow, active, (int)ray);
-    if (active && (PARTS & L4D_SC_TIME_PLANES)) {
+    l4d_bw_scatter_t<true, DfeatFromTile, false, true>(M, A.F, A.G, x, y, z, flow, df, dflow, active, (int)ray);
+    if (active) {
 #pragma unroll
       for (int k = 0; k < 6; ++k) A.sv.dflow[(size_t)k * P + p] = dflow[k];
     }

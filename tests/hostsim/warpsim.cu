@@ -60,13 +60,6 @@ static inline unsigned reduce_max(unsigned mask, unsigned v) {
   end();
   return r;
 }
-static inline int reduce_add(unsigned mask, int v) {
-  begin((uint32_t)v);
-  int r = 0;
-  for (int i = 0; i < 32; ++i) if ((mask >> i) & 1u) r += (int)t_warp->slot[i];
-  end();
-  return r;
-}
 static inline int clz(int v) { return v == 0 ? 32 : __builtin_clz((unsigned)v); }
 static inline int ffs(int v) { return __builtin_ffs(v); }
 }  // namespace ws
@@ -77,12 +70,8 @@ static inline int ffs(int v) { return __builtin_ffs(v); }
 #define __shfl_up_sync(m, v, d) ws::shfl_up((m), (v), (d))
 #define __ballot_sync(m, p) ws::ballot((m), (p))
 #define __reduce_max_sync(m, v) ws::reduce_max((m), (v))
-#define __reduce_add_sync(m, v) ws::reduce_add((m), (v))
 #define __clz(v) ws::clz((v))
 #define __ffs(v) ws::ffs((v))
-#define __float_as_uint(f) ws::f2u((f))
-#define __uint_as_float(u) ws::u2f((u))
-#define __float2int_rn(f) ((int)lrintf((f)))
 #include "../../lidar4d_b200/csrc/l4d_bwd.cuh"
 
 // ---- drivers -------------------------------------------------------------------------------------------------------------
