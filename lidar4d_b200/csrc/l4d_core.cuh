@@ -900,9 +900,11 @@ L4D_HD float l4d_attr_cdir(const DevModel& M, int net, int o, const float* enc) 
   return s;
 }
 
-// alpha of one sample (renderer.py:98-102)
+// alpha of one sample (renderer.py:98-102): 1 - exp(e), formed as -expm1(e).  On long rays alpha is ~1e-5, and
+// 1 - expf(e) would keep only the few bits of it above expf's rounding near 1; that error enters every factor of the
+// transmittance product behind the sample.
 L4D_HD float l4d_alpha(const DevModel& M, float delta, float sigma) {
   float e = M.active_sensor ? (((-2.0f * delta) * M.density_scale) * sigma)
                             : (((-delta) * M.density_scale) * sigma);
-  return 1.0f - expf(e);
+  return -expm1f(e);
 }

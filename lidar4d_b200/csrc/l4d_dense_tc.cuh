@@ -723,7 +723,7 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
           });
           // dH1[64 x 64] = dH2 * W2 on this warpgroup's rows
           mma_prop<64>(d, m0, aT3h, aT3l, 8, sb + L.wa2[net], 64);
-          float cs2;
+          float inv2;      // (1 / cs) / r: cs r can pass 2^128, where 1 / (cs r) is 0 rather than a subnormal
           {   // re-scale the propagated delta with its own amax, then dH1 * relu1 -> T2 (H2 is dead past the barrier)
             float am = 0.f;
 #pragma unroll
@@ -733,12 +733,11 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
             }
             am = block_amax256(am, s_w);
             const float r = am > 0.f ? pow2_factor(am) : 1.0f;
-            cs2 = cs * r;
+            inv2 = (1.0f / cs) / r;
 #pragma unroll
             for (int i = 0; i < 32; ++i) v[i] *= r;
             frag_put<64>(t2h, t2l, 128, m0, 0, v);
           }
-          const float inv2 = 1.0f / cs2;
           L4D_PH(4);
           publish();
           // dW1g[64 x 16] = dH1^T * [geo,1] (warpgroup w: columns [8w, 8w + 8); column 15 is the ones column)
@@ -810,7 +809,7 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
         }
         am2 = block_amax256(am2, s_w);
         const float r = am2 > 0.f ? pow2_factor(am2) : 1.0f;
-        inv = 1.0f / (sc * r);
+        inv = (1.0f / sc) / r;            // not 1 / (sc r): that is 0 once sc r passes 2^128, (1/sc)/r a subnormal to 2^149
 #pragma unroll
         for (int i = 0; i < 32; ++i) v[i] *= r;
         frag_put<64>(hh, hl, 128, m0, 0, v);
@@ -1091,14 +1090,14 @@ __global__ void __launch_bounds__(128, 2) k_bwd_flow_tc(const __grid_constant__ 
       }
     a2 = block_amax128(a2, s_w);
     float r = a2 > 0.f ? pow2_factor(a2) : 1.0f;
-    const float cs2 = sc * r;
+    const float inv2 = (1.0f / sc) / r;      // not 1 / (sc r): that is 0 once sc r passes 2^128
 #pragma unroll
     for (int mb = 0; mb < 2; ++mb) {
 #pragma unroll
       for (int i = 0; i < 32; ++i) d[mb][i] *= r;
       frag_put<64>(t1h, t1l, 128, 64 * mb, 0, d[mb]);
     }
-    inv = 1.0f / cs2;
+    inv = inv2;
     publish();
     // dH1[128 x 64] = dH2 * W1 ; dW1^T[64 x 64] = H1^T * dH2
 #pragma unroll
@@ -1117,14 +1116,13 @@ __global__ void __launch_bounds__(128, 2) k_bwd_flow_tc(const __grid_constant__ 
       }
     a3 = block_amax128(a3, s_w);
     r = a3 > 0.f ? pow2_factor(a3) : 1.0f;
-    const float cs3 = cs2 * r;
 #pragma unroll
     for (int mb = 0; mb < 2; ++mb) {
 #pragma unroll
       for (int i = 0; i < 32; ++i) d[mb][i] *= r;
       frag_put<64>(t2h, t2l, 128, 64 * mb, 0, d[mb]);
     }
-    inv = 1.0f / cs3;
+    inv = inv2 / r;
     publish();
     // dFin[128 x 16] = dH1 * W0 ; dW0[64 x 16] = dH1^T * Fin
     // dL/d(flow-MLP input) replaces the saved input in place (every thread read its row above); k_bwd_flowgrid turns it

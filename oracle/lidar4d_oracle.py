@@ -172,6 +172,33 @@ class _TruncExp(torch.autograd.Function):
 trunc_exp = _TruncExp.apply
 
 
+def _texel_axis(u: torch.Tensor, size: int):
+    """One axis of F.grid_sample(bilinear, align_corners=True, border) for a float64 coordinate u in [0, 1]: the texel
+    pair is chosen from the float32 value of the coordinate by grid_sample's float32 arithmetic, the weights are float64
+    (and differentiable).  A warped position x + flow within float32 rounding of a texel edge therefore falls in the
+    texel the float32 evaluation picks, where d(sample)/d(position) is that texel's slope."""
+    m = float(size - 1)
+    ix32 = (u.detach().float() * 2.0 - 1.0 + 1.0) / 2.0 * m
+    ix = (u * 2.0 - 1.0 + 1.0) / 2.0 * m
+    inside = (ix32 > 0.0) & (ix32 < m)                 # border padding: no gradient on or beyond the edge texels
+    ix = torch.where(inside, ix, ix.detach().clamp(0.0, m))
+    ix32 = ix32.clamp(0.0, m)
+    i0 = torch.floor(ix32).long().clamp(max=size - 1)
+    i1 = (i0 + 1).clamp(max=size - 1)
+    w1 = ix - i0.to(ix.dtype)
+    return i0, i1, 1.0 - w1, w1
+
+
+def _grid_sample_texels32(grid: torch.Tensor, cx: torch.Tensor, cy: torch.Tensor) -> torch.Tensor:
+    """Bilinear sample of grid [1, C, H, W] at (cx -> W, cy -> H) in [0, 1]: [P, C], texels selected as in float32."""
+    _, C, H, W = grid.shape
+    x0, x1, wx0, wx1 = _texel_axis(cx, W)
+    y0, y1, wy0, wy1 = _texel_axis(cy, H)
+    g = grid[0]
+    return ((g[:, y0, x0] * (wx0 * wy0) + g[:, y0, x1] * (wx1 * wy0)) +
+            (g[:, y1, x0] * (wx0 * wy1) + g[:, y1, x1] * (wx1 * wy1))).t()
+
+
 # =============================================================================
 # counter-based jitter RNG shared with the CUDA kernels (spec of this repo; the
 # reference uses torch.rand, renderer.py:84, which no other code can reproduce)
@@ -275,7 +302,8 @@ class OracleLiDAR4D(nn.Module):
         """Truth mode: parameters and all smooth arithmetic in float64.  The
         quantities the spec pins in float32 (sample positions, x01, hash cell
         selection / corner weights, the frequency-encoding argument, fp16 table
-        rounding) stay exactly as in float32, so this is the infinitely-precise
+        rounding, the plane texel that each position - warped positions x + flow included - falls in) stay exactly
+        as in float32, so this is the infinitely-precise
         evaluation of the SAME function; use it to tell which of two float32
         results is the noisy one."""
         self.double()
@@ -347,10 +375,13 @@ class OracleLiDAR4D(nn.Module):
                 if dyn != (which == "dynamic"):
                     continue
                 grid = self._plane(s, ci)
-                coords = xt[:, list(comb)].view(1, 1, -1, 2) * 2.0 - 1
-                v = F.grid_sample(grid.to(xt.dtype), coords, align_corners=True, mode="bilinear",
-                                  padding_mode="border")
-                v = v.view(grid.shape[1], -1).t()
+                if xt.dtype == torch.float64:
+                    v = _grid_sample_texels32(grid.to(xt.dtype), xt[:, comb[0]], xt[:, comb[1]])
+                else:
+                    coords = xt[:, list(comb)].view(1, 1, -1, 2) * 2.0 - 1
+                    v = F.grid_sample(grid.to(xt.dtype), coords, align_corners=True, mode="bilinear",
+                                      padding_mode="border")
+                    v = v.view(grid.shape[1], -1).t()
                 prod = v if prod is None else prod * v
             feats.append(prod)
         return torch.cat(feats, -1)

@@ -98,6 +98,15 @@ class HostSim:
         self._saved, self._fr, self._rays_s = saved, fr, rays
         return out
 
+    def saved_compositing_inputs(self):
+        """σ [N, S] and the attribute heads' outputs [2, N, S] (0 outside the attribute mask) that the last
+        render(train=True) saved, as the backward reads them."""
+        from scatter_ref import saved_layout
+        N, S = self._rays_s.n_rays, self._rays_s.n_steps
+        L = saved_layout(self.cfg, N, S)
+        f32 = lambda name, n: self._saved[L[name]:L[name] + 4 * n].view(torch.float32)
+        return dict(sigma=f32("sigma", N * S).view(N, S).clone(), attr=f32("attr", 2 * N * S).view(2, N, S).clone())
+
     def _grad_tables(self):
         grads = {k: torch.zeros_like(v) for k, v in self.params.items()}
         tab = _capi.L4DMasterGrads()
