@@ -144,13 +144,15 @@ def _texels(Pt, b):
 
 
 def scatter_reference(cfg, params: dict, frame, x01: torch.Tensor, dfeat: torch.Tensor, flow: torch.Tensor,
-                      dfin: torch.Tensor = None) -> dict:
+                      dfin: torch.Tensor = None, dfin_err: torch.Tensor = None) -> dict:
     """Float64 reference of the scatter stage.
 
     cfg FieldConfig; params: name -> fp32 master tensor (reference state_dict names); frame: geometry.FrameConstants;
     x01 [P, 3] float32 (sample_x01); dfeat [P, sigma_in_dim] float32; flow [6, P] float32 (the forward's);
-    dfin [16, P] float32 dL/d(flow-MLP input) or None (no flow-grid reference).
-    Returns name -> [numel, 3] float64 (ref, A, n) per entry in the tensor's flat order, and "dflow" -> [P, 6, 3]."""
+    dfin [16, P] dL/d(flow-MLP input) or None (no flow-grid reference): the kernel's saved float32 values, or a float64
+    reference with its error bound dfin_err [16, P] (tests/dense_ref.py, for the fp32 kernels, which never store it).
+    Returns name -> [numel, 3] float64 (ref, A, n) per entry in the tensor's flat order, and "dflow" -> [P, 6, 3]; with
+    dfin_err the flow grid's entries get a fourth column, the bound carried in from dfin_err (check_entries adds it)."""
     dev = x01.device
     P = x01.shape[0]
     nS, L = cfg.n_levels_plane, cfg.n_levels_hash
@@ -169,6 +171,7 @@ def scatter_reference(cfg, params: dict, frame, x01: torch.Tensor, dfeat: torch.
     static = _Sink(int(gs.offset[-1]) * 4, dev)
     comb = [_Sink(int(gd[p].offset[-1]), dev) for p in range(3)]        # sum of w_corner * wc * dL/dfeature
     fcomb = _Sink(int(gf.offset[-1]) * 2, dev) if dfin is not None else None
+    ferr = torch.zeros(int(gf.offset[-1]) * 2, dtype=torch.float64, device=dev) if dfin_err is not None else None
     planes, pl64 = {}, {}
     for s in range(nS):
         for ci in range(6):
@@ -205,6 +208,9 @@ def scatter_reference(cfg, params: dict, frame, x01: torch.Tensor, dfeat: torch.
                 idx, w = O.hash_indices(x, gf, l)
                 ent = ((idx + int(gf.offset[l])) * 2)[:, :, None] + torch.arange(2, device=dev)
                 fcomb.add(ent, w.double()[:, :, None] * dfi[:, None, 2 * l:2 * l + 2])
+                if ferr is not None:
+                    dfe = dfin_err[2 * l:2 * l + 2, h:h + CHUNK].t().double()
+                    ferr.index_add_(0, ent.reshape(-1), (w.double()[:, :, None] * dfe[:, None, :]).reshape(-1))
 
         for s in range(nS):
             R = cfg.min_resolution * cfg.plane_scales[s]
@@ -273,26 +279,32 @@ def scatter_reference(cfg, params: dict, frame, x01: torch.Tensor, dfeat: torch.
             out[f"hash_encoder.hash_dynamic.{p}.hash_t.{sl}.params"] = t.view(-1, 3)
     if fcomb is not None:
         ne = int(gf.offset[-1])
-        t = torch.zeros(ne, 4, 2, 3, dtype=torch.float64, device=dev)
+        nc = 3 if ferr is None else 4
+        t = torch.zeros(ne, 4, 2, nc, dtype=torch.float64, device=dev)
         fc = fcomb.t.view(ne, 2, 3)
         for i in range(4):
             bi = float(frame.flow_basis[i])
             t[:, i, :, 0] = fc[:, :, 0] * bi
             t[:, i, :, 1] = fc[:, :, 1] * abs(bi)
             t[:, i, :, 2] = fc[:, :, 2]
-        out["flow_net.grid_enc.params"] = t.view(-1, 3)
+            if ferr is not None:
+                t[:, i, :, 3] = ferr.view(ne, 2) * abs(bi)
+        out["flow_net.grid_enc.params"] = t.view(-1, nc)
     out["dflow"] = dflow
     return out
 
 
 def check_entries(got: torch.Tensor, ref: torch.Tensor, slack: int = SLACK):
-    """Per entry: |got - ref| <= (n + slack) * 2^-24 * A, and got == 0 where n == 0.
+    """Per entry: |got - ref| <= (n + slack) * 2^-24 * A (+ the carried-in bound of a fourth column), and got == 0 where
+    n == 0.
     Returns (number of failing entries, worst |got - ref| / bound, index of the worst entry)."""
     g = got.detach().reshape(-1).double()
     r, a, n = ref[..., 0].reshape(-1), ref[..., 1].reshape(-1), ref[..., 2].reshape(-1)
     assert g.numel() == r.numel(), (g.numel(), r.numel())
     err = (g - r).abs()
     bound = (n + slack) * EPS32 * a
+    if ref.shape[-1] > 3:
+        bound = bound + ref[..., 3].reshape(-1)
     bad = (err > bound) | ((n == 0) & (g != 0))
     ratio = torch.where(bound > 0, err / bound, torch.where(err > 0, torch.full_like(err, float("inf")), torch.zeros_like(err)))
     worst = int(torch.argmax(ratio))

@@ -36,9 +36,9 @@ import torch
 
 import compositing_ref as CR
 import scatter_ref as SR
-from lidar4d_b200.model import _RenderFn
 from oracle import lidar4d_oracle as O
 from parity_util import small_config, make_surface_like, cuda_model_from_oracle, test_rays as _rays
+from saved_util import train_step, saved_features
 
 pytestmark = pytest.mark.gpu
 MODES = [("tc", "split"), ("fp32", "split"), ("tc", "fused")]
@@ -85,27 +85,6 @@ def model_for(regime: str, mode: str, pipeline: str):
     return m
 
 
-def train_step(m, ro, rd, S, U, monkeypatch):
-    """Render + backward; returns the outputs and the saved buffer the backward consumed."""
-    captured = {}
-    orig = _RenderFn.backward
-
-    def keep_saved(ctx, *g):
-        captured["saved"] = ctx.saved
-        return orig(ctx, *g)
-    monkeypatch.setattr(_RenderFn, "backward", staticmethod(keep_saved))
-    m.zero_grad(set_to_none=False)
-    m._jitter_calls = 0
-    dev = next(iter(U.values())).device
-    out = m.render(ro[None].to(dev), rd[None].to(dev), torch.tensor([[0.4]]), num_steps=S, perturb=True)
-    outs = {"depth_lidar": out["depth_lidar"][0], "image_lidar": out["image_lidar"][0],
-            "weights_sum_lidar": out["weights_sum_lidar"], "weights": out["weights"]}
-    torch.autograd.backward([outs[k] for k in U], [U[k] for k in U])
-    torch.cuda.synchronize()
-    monkeypatch.undo()
-    return {k: v.detach() for k, v in out.items()}, captured["saved"]
-
-
 def sigma_jacobian(m, feat: torch.Tensor):
     """J [P, K], Ĵ [P, K] and the usable-sample mask (every hidden unit clear of its ReLU kink), float64."""
     cfg = m.cfg
@@ -121,19 +100,6 @@ def sigma_jacobian(m, feat: torch.Tensor):
     Jh = live.abs() @ W1[:, :K].abs()
     ok = ((hid.abs() > RELU_MARGIN * mag) | (w2 == 0)[None]).all(1)
     return J, Jh, ok
-
-
-def saved_features(cfg, saved: torch.Tensor, N: int, S: int, mode: str) -> torch.Tensor:
-    """The sigma MLP's input features [P, K] the dense kernels read: fp32 [K][P] (fp32 mode) or fp16 hi + lo tiles
-    [ray][tile][hi|lo][K/8][128][8] (tensor-core mode)."""
-    L = SR.saved_layout(cfg, N, S)
-    K, P = cfg.sigma_in_dim, N * S
-    if mode == "fp32":
-        return saved[L["feat"]:L["feat"] + 4 * K * P].view(torch.float32).view(K, P).t().double()
-    nt, xc = (S + 127) // 128, (K + 7) // 8
-    t = saved[L["feat"]:L["feat"] + N * nt * xc * 4096].view(torch.float16).view(N, nt, 2, xc, 128, 8).double()
-    x = (t[:, :, 0] + t[:, :, 1]).permute(0, 1, 3, 2, 4).reshape(N, nt * 128, xc * 8)
-    return x[:, :S, :K].reshape(P, K)
 
 
 def check_forward(out, ref, attr, what):

@@ -4,14 +4,16 @@ The gradient sinks of the split pipeline (k_bwd_scatter with its segmented and p
 k_fold_planes, k_fold_dynamic, k_bwd_flowgrid + k_fold_flow) make no decisions: given what they consumed - dL/dfeature
 (SavedView::dfeat), the forward's flow and, in tensor-core mode, dL/d(flow-MLP input) written over flow_in - the table
 gradients are a linear function that tests/scatter_ref.py evaluates in float64.  Every entry of every table gradient (static
-hash, every dynamic slice, all planes, the flow grid in tensor-core mode) and the saved dL/dflow of every sample is held to
+hash, every dynamic slice, all planes, the flow grid) and the saved dL/dflow of every sample is held to
 
     |got - ref| <= (n + 16) * 2^-24 * A,   got == 0 where no contribution reaches the entry,
 
 with A the sum of the contributions' magnitudes and n their count: a bound that holds whatever order the sums take, so a run
 merged over the wrong lanes, a tail lane counted twice or a fold with the wrong weight shows up even where it is far below
 1e-4 of the largest entry.  (The end-to-end oracle tests cannot be this strict: the kernels and the oracle make different
-ReLU decisions upstream.)
+ReLU decisions upstream.)  In fp32 mode k_bwd_flow scatters dL/d(flow-MLP input) into the flow grid without storing it;
+there the flow grid is held to the scatter of the float64 flow-MLP reference of tests/dense_ref.py, whose bound on
+dL/d(flow-MLP input) is carried into each entry's bound (Σ of |corner weight · basis| times it).
 
 Cases, in both MLP modes of the split pipeline:
   a. the benchmark configuration (L = 16, S = 768, jitter) at N = 2 * 16 * SMs + 37 rays, every scatter CTA wraps; rays of
@@ -29,6 +31,7 @@ import numpy as np
 import pytest
 import torch
 
+import dense_ref as DR
 import scatter_ref as SR
 from lidar4d_b200.geometry import make_frame
 from lidar4d_b200.model import _RenderFn
@@ -93,7 +96,11 @@ def assert_scatter_exact(m, ro, rd, t, S, mode, monkeypatch, what, seed=21):
     x01 = SR.sample_x01(ro.to(dev), rd.to(dev), out["z_vals"], cfg.bound)
     fr = make_frame(t, cfg.num_frames, cfg.time_resolution)
     params = {k: p.detach() for k, p in m.named_parameters()}
-    ref = SR.scatter_reference(cfg, params, fr, x01, sv["dfeat"], sv["flow"], sv["flow_in"] if mode == "tc" else None)
+    if mode == "tc":
+        dfin, dfin_err = sv["flow_in"], None
+    else:
+        dfin, dfin_err = fp32_flow_input_gradient(m, sv)
+    ref = SR.scatter_reference(cfg, params, fr, x01, sv["dfeat"], sv["flow"], dfin, dfin_err)
     grads = {k: p.grad for k, p in m.named_parameters()}
     bad, worst, touched = {}, 0.0, 0
     for k, r in ref.items():
@@ -111,6 +118,22 @@ def assert_scatter_exact(m, ro, rd, t, S, mode, monkeypatch, what, seed=21):
     print(f"[scatter-exact] {what}: {touched} touched entries + samples, worst {worst:.3f} of the bound, "
           f"max |dflow| {dflow_live:.2e}, {time.perf_counter() - t0:.1f} s")
     return out, sv, x01
+
+
+def fp32_flow_input_gradient(m, sv):
+    """The fp32 flow backward (k_bwd_flow) scatters dL/d(flow-MLP input) into the flow grid without storing it: take the
+    float64 reference of the flow MLP (tests/dense_ref.py) on the same saved input and dL/dflow, with its bound."""
+    W = DR.working_weights(m.cfg, {k: p.detach() for k, p in m.named_parameters()}, False)
+    P = sv["flow_in"].shape[1]
+    v = torch.zeros(16, P, dtype=torch.float64, device=sv["flow_in"].device)
+    e = torch.zeros_like(v)
+
+    def keep(p0, p1, o):
+        v[:, p0:p1] = o["dfin"][0].t()
+        e[:, p0:p1] = o["dfin"][1].t()
+    fref = DR.flow_reference(W, sv["flow_in"], sv["dflow"], False, keep)
+    assert fref["ambiguous"] <= 1e-2 * P, fref["ambiguous"]
+    return v, e
 
 
 def full_model(mode, seed=0):
