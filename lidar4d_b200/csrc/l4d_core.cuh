@@ -650,7 +650,9 @@ struct FeatSink {
 };
 
 #if defined(__CUDA_ARCH__)
-// features [row0, row0+n) of one sample as fp16 hi + lo (x = hi + lo to ~2^-22) into its operand tile.
+// features [row0, row0+n) of one sample as fp16 hi + lo into its operand tile: hi = fp16(x), lo = fp16(x - hi), so
+// |hi + lo - x| <= 2^-22 |x| + 2^-25.  Below |x| ~ 2^-3 the residual x - hi is an fp16 subnormal and the absolute 2^-25
+// dominates (relative error 6e-5 at |x| = 1e-3, 6e-3 at 1e-5; DESIGN.md 4.2).
 // 8-aligned groups are one 16-byte store per half (a warp writes 512 contiguous bytes), 4-aligned groups 8 bytes.
 __device__ __forceinline__ void l4d_tile_emit(unsigned char* hi, uint32_t lo_off, int row0, int n, const float* xb, int xs) {
   int i = 0;

@@ -196,7 +196,10 @@ extern "C" int hs_render_forward(const L4DConfig* cfg, const void* staged, const
       float a0 = 0.f, a1 = 0.f;
       if (w > 1e-4f) { a0 = l4d_attr_net(M, 0, cdir, geo, xb, 1); a1 = l4d_attr_net(M, 1, cdir, geo, xb, 1); }
       pd += w * zj; p0 += w * a0; p1 += w * a1; pw += w;
-      if (saved) { sv.sigma[p] = sigma; sv.attr[p] = a0; sv.attr[sv.P + p] = a1; }
+      if (saved) {      // flow as the split pipeline saves it (the warped positions of the sample)
+        sv.sigma[p] = sigma; sv.attr[p] = a0; sv.attr[sv.P + p] = a1;
+        for (int k = 0; k < 6; ++k) sv.flow[(size_t)k * sv.P + p] = fl[k];
+      }
       if (weights) weights[p] = w;
       if (zvals) zvals[p] = zj;
     }

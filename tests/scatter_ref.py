@@ -67,17 +67,39 @@ def saved_layout(cfg, n_rays: int, S: int) -> dict:
 
 
 def decode_saved(cfg, saved: torch.Tensor, n_rays: int, S: int) -> dict:
-    """Views of the saved buffer (uint8) that the scatter stage reads or writes:
-    dfeat [P, sigma_in_dim] (from the tiles [ray][tile][k/4][128][4]), flow / dflow [6, P], flow_in [16, P]."""
+    """Views of the saved buffer (uint8) that the split pipeline's stages read or write:
+    dfeat [P, sigma_in_dim] (from the tiles [ray][tile][k/4][128][4]), flow / dflow [6, P], flow_in [16, P];
+    the features, as fp32 SoA planes feat [sigma_in_dim, P] (fp32 mode) or as the raw fp16 operand tiles
+    feat_tiles [ray][tile][hi|lo][k/8][128][8] (tensor-core mode; both views cover the same bytes);
+    hd_con[q][p] [entries] (the contracted dynamic tables of query q = cur|fwd|bwd and plane p) and
+    pl_con[q][s][t] [R, 8] (the contracted time-plane rows of query q, scale s, time plane t = (x,t)|(y,t)|(z,t))."""
     L = saved_layout(cfg, n_rays, S)
     assert saved.numel() >= L["total"], (saved.numel(), L["total"])
     P = n_rays * S
-    f32 = lambda name, n: saved[L[name]:L[name] + 4 * n].view(torch.float32)
-    nt, dq = (S + 127) // 128, (cfg.sigma_in_dim + 3) // 4
+    f32 = lambda name, n, o=0: saved[L[name] + 4 * o:L[name] + 4 * (o + n)].view(torch.float32)
+    nt, dq, xc = (S + 127) // 128, (cfg.sigma_in_dim + 3) // 4, (cfg.sigma_in_dim + 7) // 8
     df = f32("dfeat", n_rays * nt * dq * 128 * 4).view(n_rays, nt, dq, 128, 4)
     df = df.permute(0, 1, 3, 2, 4).reshape(n_rays, nt * 128, dq * 4)[:, :S, :cfg.sigma_in_dim].reshape(P, -1)
+    tiles = saved[L["feat"]:L["feat"] + n_rays * nt * xc * 4096].view(torch.float16).view(n_rays, nt, 2, xc, 128, 8)
+    ne = [int(cfg.dynamic_grid(p).offset[-1]) for p in range(3)]
+    hd, o = [], 0
+    for q in range(3):
+        hd.append([])
+        for p in range(3):
+            hd[q].append(f32("hd_con", ne[p], o))
+            o += ne[p]
+    pl, o = [], 0
+    for q in range(3):
+        pl.append([])
+        for s in range(cfg.n_levels_plane):
+            R = cfg.min_resolution * cfg.plane_scales[s]
+            pl[q].append([])
+            for t in range(3):
+                pl[q][s].append(f32("pl_con", R * 8, o).view(R, 8))
+                o += R * 8
     return dict(dfeat=df, flow=f32("flow", 6 * P).view(6, P), dflow=f32("dflow", 6 * P).view(6, P),
-                flow_in=f32("flow_in", 16 * P).view(16, P))
+                flow_in=f32("flow_in", 16 * P).view(16, P), feat=f32("feat", cfg.sigma_in_dim * P).view(-1, P),
+                feat_tiles=tiles, hd_con=hd, pl_con=pl)
 
 
 # ---- the kernels' float32 position arithmetic ---------------------------------------------------------------------------
