@@ -477,6 +477,32 @@ int    l4d_sweep_images(const float* depth, const float* image, const void* rayd
                         const uint8_t* lut_intensity, const uint8_t* lut_depth, uint8_t* panel, float* pano_or_null,
                         float* intensities_or_null, void* stream);
 
+/* --- the ray-drop refinement loop (model/runner.py Trainer.refine:865-913) ---------------------------------------------
+ * l4d_box_mask: out = x * m over x[B, C, H, W] float32 (out may alias x), with m = 0 inside any of the n_boxes <=
+ *   L4D_MAX_BOXES boxes and 1 elsewhere, the same for every batch item and channel.  boxes is a HOST int32 array
+ *   [n_boxes, 4] of (y0, x0, h, w) with h, w >= 1, y0, x0 >= 0, y0 + h <= H and x0 + w <= W (it may be NULL when
+ *   n_boxes = 0); it is passed to the kernel by value, so there is no copy and no sync.  The mask is multiplied, not
+ *   selected: a negative x in a box gives -0.0, an inf or NaN in a box gives NaN.  B*C*H*W < 2^31.  One launch.
+ * l4d_bce_loss = torch.nn.BCELoss() (mean reduction): pred[n] of dtype L4D_DTYPE_*, target[n] float32, 1 <= n < 2^31,
+ *   each element in float32 as ((t - 1) * max(log1p(-x), -100)) - (t * max(log(x), -100)).  A pred outside [0, 1] or NaN
+ *   gives a NaN element (torch's CUDA kernel asserts instead).  WRITES *loss (device float) = float32(sum / n) with the
+ *   sum taken in double in a fixed order.  work = l4d_bce_loss_work_bytes() bytes (L4D_ESIZE when smaller).  Two
+ *   launches (the partial sums, then a one-CTA finish).
+ * l4d_bce_loss_backward: g_pred[n], in pred's dtype, = ((*g_loss * (x - t)) / max((1 - x) * x, 1e-12)) / n in float32,
+ *   torch's gradient; NaN where pred is outside [0, 1] or NaN.  *g_loss is read from device memory.  One launch.
+ * Null required pointers, bad sizes, dtypes, box counts or boxes: L4D_EINVAL. */
+#define L4D_MAX_BOXES 32
+#define L4D_DTYPE_F32  0u
+#define L4D_DTYPE_F16  1u
+#define L4D_DTYPE_BF16 2u
+int    l4d_box_mask(const float* x, float* out, uint32_t B, uint32_t C, uint32_t H, uint32_t W, const int32_t* boxes_or_null,
+                    uint32_t n_boxes, void* stream);
+size_t l4d_bce_loss_work_bytes(void);
+int    l4d_bce_loss(const void* pred, uint32_t pred_dtype, const float* target, uint32_t n, float* loss, void* work,
+                    size_t work_bytes, void* stream);
+int    l4d_bce_loss_backward(const void* pred, uint32_t pred_dtype, const float* target, uint32_t n, const float* g_loss,
+                             void* g_pred, void* stream);
+
 /* --- profiling aid: while started, CUDA events are recorded on the launch stream around every kernel of
  *     l4d_render_forward / l4d_render_backward.  l4d_profile_stop returns the number of (kernel name, ms)
  *     pairs written (static strings), or a negative error code.  Not thread-safe. --------------------------- */

@@ -158,9 +158,13 @@ EXPORTS = [
     "l4d_flow_term_backward", "l4d_flow_ground", "l4d_flow_ground_backward", "l4d_flow_loss_finish",
     "l4d_image_metrics_work_bytes", "l4d_image_metrics", "l4d_raydrop_metrics",
     "l4d_sweep_images",
+    "l4d_box_mask", "l4d_bce_loss_work_bytes", "l4d_bce_loss", "l4d_bce_loss_backward",
 ]
 SWEEP_SIM, SWEEP_TEST, SWEEP_EVAL = 0, 1, 2     # L4D_SWEEP_* layouts of l4d_sweep_images
 SWEEP_F32, SWEEP_F16 = 0, 1                     # L4D_SWEEP_* ray-drop dtypes
+MAX_BOXES = 32                                  # L4D_MAX_BOXES of l4d_box_mask
+DTYPE_F32, DTYPE_F16, DTYPE_BF16 = 0, 1, 2      # L4D_DTYPE_* of l4d_bce_loss
+EINVAL = -1                                     # L4D_EINVAL
 
 
 def lib_path() -> str:
@@ -266,6 +270,13 @@ def declare(lib, prefix: str = "l4d_", host_sim: bool = False):
         lib.l4d_raydrop_metrics.restype = C.c_int
         lib.l4d_sweep_images.argtypes = [V, V, V, U32, U32, U32, U32, C.c_float, U32, V, V, V, V, V, V]
         lib.l4d_sweep_images.restype = C.c_int
+        lib.l4d_box_mask.argtypes = [V, V, U32, U32, U32, U32, V, U32, V]
+        lib.l4d_bce_loss_work_bytes.argtypes = []
+        lib.l4d_bce_loss_work_bytes.restype = SZ
+        lib.l4d_bce_loss.argtypes = [V, U32, V, U32, V, V, SZ, V]
+        lib.l4d_bce_loss_backward.argtypes = [V, U32, V, U32, V, V, V]
+        for n in ("box_mask", "bce_loss", "bce_loss_backward"):
+            getattr(lib, f"l4d_{n}").restype = C.c_int
         D, F = C.c_double, C.c_float
         for n in ("range_filter", "outlier_select", "ground_split"):
             getattr(lib, f"l4d_{n}_work_bytes").argtypes = [U32]

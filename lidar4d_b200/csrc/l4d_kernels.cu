@@ -19,6 +19,7 @@
 #include "l4d_nngrid.cuh"
 #include "l4d_imgmetrics.cuh"
 #include "l4d_sweep.cuh"
+#include "l4d_refine.cuh"
 
 // =============================================================================
 // error plumbing
@@ -1825,6 +1826,78 @@ extern "C" int l4d_sweep_images(const float* depth, const float* image, const vo
   A.test_mask = test_mask != 0;
   A.scale = scale;
   ++g_launches; k_sweep_images<<<nblk(A.hw, L4D_SWEEP_NT), L4D_SWEEP_NT, 0, (cudaStream_t)stream>>>(A);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+// =============================================================================
+// box masking and the BCE loss of the ray-drop refinement loop (l4d_refine.cuh)
+// =============================================================================
+extern "C" int l4d_box_mask(const float* x, float* out, uint32_t B, uint32_t C, uint32_t H, uint32_t W, const int32_t* boxes,
+                            uint32_t n_boxes, void* stream) {
+  if (!x || !out) return l4d_fail(L4D_EINVAL, "l4d_box_mask: null pointer");
+  if (B == 0 || C == 0 || H == 0 || W == 0 || (uint64_t)B * C * H * W >= (1ull << 31))
+    return l4d_fail(L4D_EINVAL, "l4d_box_mask: need 1 <= B, C, H, W and B*C*H*W < 2^31");
+  if (n_boxes > L4D_MAX_BOXES) return l4d_fail(L4D_EINVAL, "l4d_box_mask: more than 32 boxes");
+  if (n_boxes && !boxes) return l4d_fail(L4D_EINVAL, "l4d_box_mask: null boxes");
+  L4DBoxes b;
+  b.n = n_boxes;
+  for (uint32_t k = 0; k < n_boxes; ++k) {
+    const int32_t y0 = boxes[4 * k], x0 = boxes[4 * k + 1], h = boxes[4 * k + 2], w = boxes[4 * k + 3];
+    if (y0 < 0 || x0 < 0 || h < 1 || w < 1 || (int64_t)y0 + h > (int64_t)H || (int64_t)x0 + w > (int64_t)W)
+      return l4d_fail(L4D_EINVAL, "l4d_box_mask: box outside the image or empty (need y0, x0 >= 0, h, w >= 1, y0+h <= H, x0+w <= W)");
+    b.y0[k] = y0; b.x0[k] = x0; b.h[k] = h; b.w[k] = w;
+  }
+  const uint32_t planes = B * C;
+  const dim3 grid((H * W + L4D_BOX_NT - 1) / L4D_BOX_NT, (planes + L4D_BOX_PLANES - 1) / L4D_BOX_PLANES);
+  if (grid.y > 65535) return l4d_fail(L4D_EINVAL, "l4d_box_mask: B*C too large");
+  ++g_launches; k_box_mask<<<grid, L4D_BOX_NT, 0, (cudaStream_t)stream>>>(x, out, planes, H, W, b);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+extern "C" size_t l4d_bce_loss_work_bytes(void) { return sizeof(L4DBceWork); }
+
+static int bce_check(const void* pred, uint32_t dtype, const float* target, uint32_t n, const char* who) {
+  if (!pred || !target) return l4d_fail(L4D_EINVAL, "%s: null pointer", who);
+  if (dtype > L4D_DTYPE_BF16) return l4d_fail(L4D_EINVAL, "%s: unknown pred dtype", who);
+  if (n == 0 || n >= (1u << 31)) return l4d_fail(L4D_EINVAL, "%s: need 1 <= n < 2^31", who);
+  return L4D_OK;
+}
+
+extern "C" int l4d_bce_loss(const void* pred, uint32_t dtype, const float* target, uint32_t n, float* loss, void* work,
+                            size_t work_bytes, void* stream) {
+  if (int rc = bce_check(pred, dtype, target, n, "l4d_bce_loss")) return rc;
+  if (!loss || !work) return l4d_fail(L4D_EINVAL, "l4d_bce_loss: null pointer");
+  if (work_bytes < sizeof(L4DBceWork)) return l4d_fail(L4D_ESIZE, "l4d_bce_loss: work buffer too small");
+  const size_t per = (size_t)L4D_BCE_NT * L4D_BCE_PER_THREAD;
+  const uint32_t parts = (uint32_t)((n + per - 1) / per < L4D_BCE_BLOCKS ? (n + per - 1) / per : L4D_BCE_BLOCKS);
+  cudaStream_t st = (cudaStream_t)stream;
+  L4DBceWork* wk = (L4DBceWork*)work;
+  ++g_launches;
+  if (dtype == L4D_DTYPE_F16) k_bce<__half><<<parts, L4D_BCE_NT, 0, st>>>((const __half*)pred, target, n, wk);
+  else if (dtype == L4D_DTYPE_BF16) k_bce<__nv_bfloat16><<<parts, L4D_BCE_NT, 0, st>>>((const __nv_bfloat16*)pred, target, n, wk);
+  else k_bce<float><<<parts, L4D_BCE_NT, 0, st>>>((const float*)pred, target, n, wk);
+  L4D_CUDA(cudaGetLastError());
+  ++g_launches; k_bce_finish<<<1, 1024, 0, st>>>(wk, parts, n, loss);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+extern "C" int l4d_bce_loss_backward(const void* pred, uint32_t dtype, const float* target, uint32_t n, const float* g_loss,
+                                     void* g_pred, void* stream) {
+  if (int rc = bce_check(pred, dtype, target, n, "l4d_bce_loss_backward")) return rc;
+  if (!g_loss || !g_pred) return l4d_fail(L4D_EINVAL, "l4d_bce_loss_backward: null pointer");
+  int grid = nblk(n);
+  if (grid > 8 * sm_count()) grid = 8 * sm_count();
+  cudaStream_t st = (cudaStream_t)stream;
+  ++g_launches;
+  if (dtype == L4D_DTYPE_F16)
+    k_bce_bwd<__half><<<grid, 256, 0, st>>>((const __half*)pred, target, n, g_loss, (__half*)g_pred);
+  else if (dtype == L4D_DTYPE_BF16)
+    k_bce_bwd<__nv_bfloat16><<<grid, 256, 0, st>>>((const __nv_bfloat16*)pred, target, n, g_loss, (__nv_bfloat16*)g_pred);
+  else
+    k_bce_bwd<float><<<grid, 256, 0, st>>>((const float*)pred, target, n, g_loss, (float*)g_pred);
   L4D_CUDA(cudaGetLastError());
   return L4D_OK;
 }

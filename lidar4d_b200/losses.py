@@ -13,6 +13,10 @@ gradient from device memory (a GradScaler-scaled backward needs no host sync):
     loss = loss + line_of_sight_loss(out["weights"], out["z_vals"], gt, eps)        # --urf_loss
     loss = loss + lidar_patch_loss(out["depth_lidar"], gt, **vars(opt))             # patch batches
 
+and the ray-drop refinement loop's BCE (model/runner.py:901; the loop itself is lidar4d_b200/refine.py):
+
+    loss = raydrop_bce_loss(unet(masked_input), gt_raydrop)
+
 Inputs are taken in fp32 whatever the surrounding autocast (the reference's Sobel conv2d runs in fp16 under its fp16
 autocast; here it runs in fp32).  No CPU path."""
 from __future__ import annotations
@@ -91,6 +95,55 @@ class _PatchLoss(torch.autograd.Function):
             rc = lib.l4d_patch_loss_backward(gd.data_ptr(), gl.data_ptr(), gd.numel(), out.data_ptr(), _stream(gd))
         _capi.check(lib, rc, "l4d_patch_loss_backward")
         return (out.view(ctx.shape),) + (None,) * 10
+
+
+_BCE_DTYPES = {torch.float32: _capi.DTYPE_F32, torch.float16: _capi.DTYPE_F16, torch.bfloat16: _capi.DTYPE_BF16}
+
+
+class _RaydropBCE(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, pred, target):
+        lib = _capi.load_library()
+        p = pred.detach().contiguous()
+        t = target.detach().contiguous().float()
+        loss = torch.empty((), device=p.device)
+        work = torch.empty(lib.l4d_bce_loss_work_bytes(), dtype=torch.uint8, device=p.device)
+        with torch.cuda.device(p.device):
+            rc = lib.l4d_bce_loss(p.data_ptr(), _BCE_DTYPES[p.dtype], t.data_ptr(), p.numel(), loss.data_ptr(),
+                                  work.data_ptr(), work.numel(), _stream(p))
+        _capi.check(lib, rc, "l4d_bce_loss")
+        ctx.save_for_backward(p, t)
+        ctx.shape = pred.shape
+        return loss
+
+    @staticmethod
+    def backward(ctx, gl):
+        p, t = ctx.saved_tensors
+        lib = _capi.load_library()
+        gl = gl.detach().float().contiguous()
+        out = torch.empty_like(p)
+        with torch.cuda.device(p.device):
+            rc = lib.l4d_bce_loss_backward(p.data_ptr(), _BCE_DTYPES[p.dtype], t.data_ptr(), p.numel(), gl.data_ptr(),
+                                           out.data_ptr(), _stream(p))
+        _capi.check(lib, rc, "l4d_bce_loss_backward")
+        return out.view(ctx.shape), None
+
+
+def raydrop_bce_loss(pred, target):
+    """model/runner.py:901, ``torch.nn.BCELoss()(pred, target)`` (mean), as a device scalar with no host read, forward or
+    backward.  pred is float32, float16 or bfloat16 (the U-Net's output under any autocast), target any float dtype, read
+    as float32; the elements are computed in float32 and summed in double in a fixed order.  The gradient (pred's dtype)
+    is torch's.  Unlike torch, which fires a device-side assert, a pred outside [0, 1] or NaN makes the loss NaN (and
+    that element's gradient NaN).  No gradient flows to target."""
+    if not (pred.is_cuda and target.is_cuda):
+        raise RuntimeError("raydrop_bce_loss runs on CUDA only (no CPU fallback)")
+    if pred.dtype not in _BCE_DTYPES:
+        raise ValueError(f"pred must be float32, float16 or bfloat16, got {pred.dtype}")
+    if target.shape != pred.shape:
+        raise ValueError(f"target {tuple(target.shape)} and pred {tuple(pred.shape)} must have the same shape")
+    if pred.numel() == 0:
+        raise ValueError("raydrop_bce_loss of an empty tensor")
+    return _RaydropBCE.apply(pred, target)
 
 
 def lidar_patch_loss(depth, gt, patch_size, scale, depth_grad_loss="l1", sobel_grad=False, grad_loss=True, alpha_grad=0.1,
