@@ -219,6 +219,12 @@ int    l4d_render_backward_ex(const L4DConfig* cfg, const void* staged, const L4
                               const float* g_wsum_or_null, const float* g_weights_or_null,
                               const L4DMasterGrads* grads, void* grad_work, size_t grad_work_bytes,
                               void* ev_hash_done_or_null, void* stream);
+/* The compositing backward of the tensor-core split pipeline alone (the first kernel l4d_render_backward runs there), on
+ * the saved buffer of a training forward: afterwards feature columns 0..3 of the saved dL/dfeature hold dL/dsigma,
+ * dL/da0, dL/da1 and the attribute mask (0 / 1) of every sample.  Tensor-core configurations only (L4D_EINVAL else). */
+int    l4d_composite_backward(const L4DConfig* cfg, const L4DRays* rays, void* saved, size_t saved_bytes,
+                              const float* g_depth, const float* g_image,
+                              const float* g_wsum_or_null, const float* g_weights_or_null, void* stream);
 int    l4d_unstage_grads(const L4DConfig* cfg, const void* grad_work, size_t grad_work_bytes,
                          const L4DMasterGrads* grads, void* stream);
 

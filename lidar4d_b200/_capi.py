@@ -159,6 +159,7 @@ EXPORTS = [
     "l4d_image_metrics_work_bytes", "l4d_image_metrics", "l4d_raydrop_metrics",
     "l4d_sweep_images",
     "l4d_box_mask", "l4d_bce_loss_work_bytes", "l4d_bce_loss", "l4d_bce_loss_backward",
+    "l4d_composite_backward",
 ]
 SWEEP_SIM, SWEEP_TEST, SWEEP_EVAL = 0, 1, 2     # L4D_SWEEP_* layouts of l4d_sweep_images
 SWEEP_F32, SWEEP_F16 = 0, 1                     # L4D_SWEEP_* ray-drop dtypes
@@ -195,6 +196,9 @@ def declare(lib, prefix: str = "l4d_", host_sim: bool = False):
         lib.l4d_render_backward_ex.argtypes = [P(L4DConfig), V, P(L4DFrame), P(L4DRays), V, SZ, V, V, V, V,
                                                P(L4DMasterGrads), V, SZ, V, V]
         lib.l4d_render_backward_ex.restype = C.c_int
+        # the tensor-core pipeline's compositing backward alone (per-sample dL/dsigma, dL/da, mask -> saved dL/dfeature)
+        lib.l4d_composite_backward.argtypes = [P(L4DConfig), P(L4DRays), V, SZ, V, V, V, V, V]
+        lib.l4d_composite_backward.restype = C.c_int
         f("unstage_grads").argtypes = [P(L4DConfig), V, SZ, P(L4DMasterGrads), V]
         f("flow_forward").argtypes = [P(L4DConfig), V, P(L4DFrame), V, U32, V, V, V]
         f("flow_backward").argtypes = [P(L4DConfig), V, P(L4DFrame), V, U32, V, V, P(L4DMasterGrads), V, SZ, V]

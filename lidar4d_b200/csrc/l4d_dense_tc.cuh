@@ -147,13 +147,14 @@ __host__ __device__ inline DenseFwdSmem dense_fwd_smem(uint32_t in_pad) {
 // loss-scaled or tiny upstream gradients neither overflow nor flush; the scale is undone when the
 // fp32 accumulators are read back.  Weight-gradient accumulators are flushed from the registers with fp32
 // atomics once per tile (same count as the FMA kernel's tile_outer_accum).
-// Shared memory at sigma_in_pad = 176 (L = 16): 196 KB; one CTA per SM.
+// Shared memory at sigma_in_pad = 176 (L = 16): 217 KB; one CTA per SM.
 // =============================================================================================
 struct DenseBwdSmem {
   uint32_t w1, w2, wa1[2], wa2[2];
   uint32_t R;            // 96 KB: X hi|lo (24 chunks each) or T1,T2,T3 (hi|lo, 8 chunks each)
   uint32_t RH;           // 32 KB: sigma hidden hi|lo, later its delta
   uint32_t g16, do16, do8;   // small tiles, hi|lo
+  uint32_t slab2, slab1;     // attribute weight-gradient partials of warpgroup 1 (fp32, fragment order): dW2 + dw3, dW1g
   uint32_t misc;
   uint32_t total;
 };
@@ -166,7 +167,8 @@ __host__ __device__ inline DenseBwdSmem dense_bwd_smem(uint32_t in_pad) {
   L.wa2[0] = take(64 * 64 * 2); L.wa2[1] = take(64 * 64 * 2);
   L.R = take(96 * 1024); L.RH = take(32 * 1024);
   L.g16 = take(2 * 4096); L.do16 = take(2 * 4096); L.do8 = take(2 * 2048);
-  L.misc = take((80 + 128 + 128 + 128 + 32 + 64 + 128 + 256 + 128) * 4);
+  L.slab2 = take((32 + 2) * 128 * 4); L.slab1 = take(8 * 128 * 4);
+  L.misc = take((80 + 128 + 128 + 128 + 32 + 128 + 256 + 128) * 4);
   L.total = o;
   return L;
 }
@@ -181,6 +183,14 @@ __device__ __forceinline__ void mma_tt(uint32_t a_hi, uint32_t a_lo, uint32_t b_
   float d[N / 2];
   wg_gemm<N, 1, 1>(d, a, b, 3, 8);
   frag_foreach<N>(d, f);
+}
+// the same product over the 64 samples [m0, m0 + 64) only, issued as one wgmma group; the caller waits
+template <int N>
+__device__ __forceinline__ void mma_tt64_issue(float (&d)[N / 2], int m0, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
+  const uint32_t o = (uint32_t)m0 * 16u;
+  const Opnd a{{a_hi + o, a_lo + o, a_hi + o}, 256u, 128u, 2048u};
+  const Opnd b{{b_hi + o, b_hi + o, b_lo + o}, 256u, 128u, 2048u};
+  wg_gemm_issue<N, 1, 1>(d, a, b, 3, 4);
 }
 __device__ __forceinline__ void red2(float* p, float a, float b) { atomicAdd(reinterpret_cast<float2*>(p), make_float2(a, b)); }
 __device__ __forceinline__ float block_amax128(float v, float* s_w) {
@@ -252,6 +262,22 @@ __device__ __forceinline__ float half_excl_suffix_sum(float v, float* s_w, float
   __syncthreads();
   return post + ex;
 }
+// max |v| over the 128 threads of this thread's warpgroup (s_w[4 wg .. 4 wg + 3])
+__device__ __forceinline__ float wg_amax(float v, float* s_w) {
+  const int warp = threadIdx.x >> 5, base = warp & 4;
+  v = fabsf(v);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  if ((threadIdx.x & 31) == 0) s_w[warp] = v;
+  wg_bar();
+  const float r = fmaxf(fmaxf(s_w[base], s_w[base + 1]), fmaxf(s_w[base + 2], s_w[base + 3]));
+  wg_bar();
+  return r;
+}
+// producer / consumer handshake between the two warpgroups of a 256-thread CTA on named barrier id: one warpgroup
+// arrives (does not wait), the other waits for it
+__device__ __forceinline__ void pair_arrive(int id) { asm volatile("bar.arrive %0, 256;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ void pair_wait(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
 __device__ __forceinline__ float block_amax256(float v, float* s_w) {
   v = fabsf(v);
 #pragma unroll
@@ -466,10 +492,59 @@ __device__ unsigned long long g_phase_clk[32];
 #define L4D_PH(i) do { } while (0)
 #endif
 
-// 256 threads: warpgroup w computes rows [64w, 64w + 64) of every row-wise product and runs its epilogues on the
-// fragments; the compositing scans run in row order (two threads per row) and hand their per-row results to the
-// fragments through small per-row arrays.  The per-tile gradient scales and the weight-gradient products (K = 128
-// samples) still couple the two warpgroups at every delta tile.
+// backward 0/3: the compositing backward of the tensor-core pipeline.  One 128-thread CTA per ray (thread == row of a
+// tile) walks the tiles back to front with the carried suffix sum and leaves {dL/dsigma, dL/da0, dL/da1, attribute mask
+// (0 / 1)} of every sample in quad 0 of the sample's row of the dL/dfeature tile.  k_bwd_dense_tc reads them at the
+// start of the tile and overwrites them with dL/dfeature at its end.  The scans are the forward's (half_excl_prod over
+// four warps from the saved transmittance at the tile start), the per-sample arithmetic that of the FMA kernels.
+__global__ void __launch_bounds__(128) k_bwd_composite(const __grid_constant__ SplitArgs A) {
+  using namespace l4dtc;
+  __shared__ float s_w[8];
+  const DevModel& M = A.M;
+  const int row = threadIdx.x;
+  const RaySampling rs = l4d_make_sampling(M.near_lidar, M.far_lidar, A.S, A.perturb, A.seed);
+  const uint32_t n_steps = A.S;
+  const int n_tiles = (int)A.sv.n_tiles;
+  const float kk = M.active_sensor ? 2.0f : 1.0f;
+  for (uint32_t ray = blockIdx.x; ray < A.n_rays; ray += gridDim.x) {
+    const float gd = __ldg(A.g_depth + ray), gi0 = __ldg(A.g_image + 2 * ray), gi1 = __ldg(A.g_image + 2 * ray + 1);
+    const float gws = A.g_wsum ? __ldg(A.g_wsum + ray) : 0.f;
+    const uint64_t rg = A.ray_offset + ray;
+    float suffix = 0.f;
+    for (int t = n_tiles - 1; t >= 0; --t) {
+      const uint32_t j = (uint32_t)t * 128 + row;
+      const bool active = j < n_steps;
+      const size_t p = (size_t)ray * n_steps + (active ? j : 0);
+      float v = 1.f, alpha = 0.f, gw = 0.f, delta = 0.f;
+      if (active) {
+        const float zj = l4d_z(rs, rg, j);
+        delta = (j + 1 < n_steps) ? (l4d_z(rs, rg, j + 1) - zj) : rs.sample_dist;
+        alpha = l4d_alpha(M, delta, A.sv.sigma[p]);
+        v = (1.0f - alpha) + 1e-15f;
+        gw = gd * zj + gi0 * A.sv.attr[p] + gi1 * A.sv.attr[A.sv.P + p] + gws;
+        if (A.g_weights) gw += __ldg(A.g_weights + p);
+      }
+      float total, qtot;
+      const float T = __ldg(A.sv.tstart + (size_t)ray * n_tiles + t) * half_excl_prod(v, s_w, total);
+      const float w = alpha * T;
+      const float suf = suffix + half_excl_suffix_sum(gw * w, s_w, qtot);
+      suffix += qtot;
+      if (active) {
+        const float dsigma = (gw * T - suf / v) * (kk * delta * M.density_scale) * (1.0f - alpha);
+        const bool masked = w > 1e-4f;
+        *reinterpret_cast<float4*>(A.sv.dfeat + l4d_dfeat_off(A.sv, ray, j)) =
+            masked ? make_float4(dsigma, w * gi0, w * gi1, 1.f) : make_float4(dsigma, 0.f, 0.f, 0.f);
+      }
+    }
+  }
+}
+
+// backward 1/3 on tensor cores.  256 threads: warpgroup w owns rows [64w, 64w + 64) of every tile and computes them in
+// every row-wise product, running its epilogues on the fragments.  In the attribute heads the warpgroups run apart:
+// each skips a head whose rows carry no gradient, scales its delta tiles by its own 64-row amax and forms the weight
+// gradients of its own 64 samples; where both ran a head, warpgroup 1 hands its (unscaled) partials to warpgroup 0
+// through a shared-memory slab and warpgroup 0 issues the reductions, so every weight gradient is still reduced once per
+// 128-sample tile.  The sigma-MLP phases (P1, P3, P4) synchronise the CTA as before.
 __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ SplitArgs A) {
   using namespace l4dtc;
   extern __shared__ __align__(128) unsigned char dsm[];
@@ -501,12 +576,21 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
   float* s_cdir2 = s_cdir + 128;   // same minus the first ones-row (the tile's column 15 carries that 1)
   float* s_csum = s_cdir2 + 128;
   float* s_w = s_csum + 128;
-  float* s_tstart = s_w + 32;
-  float* s_dsig = s_tstart + 64;   // per row: dL/dsigma, attribute deltas of both heads, attribute mask (0 / 1)
+  float* s_dsig = s_w + 32;        // per row: dL/dsigma, attribute deltas of both heads, attribute mask (0 / 1)
   float* s_da = s_dsig + 128;
   float* s_mk = s_da + 256;
+  float* slab2 = reinterpret_cast<float*>(dsm + L.slab2);
+  float* slab1 = reinterpret_cast<float*>(dsm + L.slab1);
   const int m0 = 64 * wg;          // rows of this warpgroup
+  const int lt = tid & 127;        // thread within the warpgroup (slab index)
   __shared__ float s_w3max[2];
+  // per tile (two slots, by the parity of the CTA's tile count): bit 2 w + net = rows of warpgroup w carry a gradient
+  // for attribute head net
+  __shared__ uint32_t s_heads[2];
+  uint32_t tile_no = 0;
+  // warpgroup 1: a slab holds partials warpgroup 0 has not consumed yet (named barriers 3 / 4: slab2 full / free,
+  // 5 / 6: slab1 full / free)
+  bool slab2_busy = false, slab1_busy = false;
 #ifdef L4D_PHASE_CLOCKS
   __shared__ unsigned long long s_clk[32];
   long long t_last = clock64();
@@ -532,11 +616,10 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
     cp(L.wa2[0], M.tc_att_w2[0], 64 * 64 * 2);
     cp(L.wa2[1], M.tc_att_w2[1], 64 * 64 * 2);
   }
+  if (tid < 2) s_heads[tid] = 0u;
   publish();
-  const RaySampling rs = l4d_make_sampling(M.near_lidar, M.far_lidar, A.S, A.perturb, A.seed);
   const uint32_t n_steps = A.S;
   const int n_tiles = (int)((n_steps + 127) / 128);
-  const float kk = M.active_sensor ? 2.0f : 1.0f;
   const int n_xchunks = (int)in_pad / 8;
 
   // The X tile (fp16 hi|lo operand tile written by k_fwd_gather) arrives by bulk copy.  It is needed twice per tile
@@ -573,9 +656,6 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
 
   for (uint32_t ray = blockIdx.x; ray < A.n_rays; ray += gridDim.x) {
     const float dx = __ldg(A.rays_d + 3 * ray), dy = __ldg(A.rays_d + 3 * ray + 1), dz = __ldg(A.rays_d + 3 * ray + 2);
-    const float gd = __ldg(A.g_depth + ray), gi0 = __ldg(A.g_image + 2 * ray), gi1 = __ldg(A.g_image + 2 * ray + 1);
-    const float gws = A.g_wsum ? __ldg(A.g_wsum + ray) : 0.f;
-    const uint64_t rg = A.ray_offset + ray;
     __syncthreads();
     for (int i = tid; i < L4D_ENC; i += 256) {
       const int dim = i / 24, k = (i % 24) >> 1, ph = i & 1;
@@ -588,44 +668,22 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
       s_cdir[tid] = c;
       s_cdir2[tid] = c - l4d_ld1(M.att_w1t[tid >> 6] + (size_t)M.attr_in_dim * L4D_H + (tid & 63));
     }
-    __syncthreads();
-    // transmittance at the start of every tile: saved by k_fwd_dense_tc
-    for (int t = tid; t < n_tiles; t += 256) s_tstart[t] = __ldg(A.sv.tstart + (size_t)ray * A.sv.n_tiles + t);
-    __syncthreads();
     L4D_PH(0);
-    float suffix = 0.f;
     for (int t = n_tiles - 1; t >= 0; --t) {
       const uint32_t j = (uint32_t)t * 128 + row;
       const bool active = j < n_steps;
-      const size_t p = (size_t)ray * n_steps + (active ? j : 0);
-      bool masked = false;
-      float dsigma = 0.f, da[2] = {0.f, 0.f};
-      {
-        float v = 1.f, alpha = 0.f, gw = 0.f, delta = 0.f;
-        if (active) {
-          const float zj = l4d_z(rs, rg, j);
-          delta = (j + 1 < n_steps) ? (l4d_z(rs, rg, j + 1) - zj) : rs.sample_dist;
-          alpha = l4d_alpha(M, delta, A.sv.sigma[p]);
-          v = (1.0f - alpha) + 1e-15f;
-          gw = gd * zj + gi0 * A.sv.attr[p] + gi1 * A.sv.attr[A.sv.P + p] + gws;
-          if (A.g_weights) gw += __ldg(A.g_weights + p);
-        }
-        float total, qtot;
-        const float T = s_tstart[t] * half_excl_prod(v, s_w, total);
-        const float w = alpha * T;
-        const float suf = suffix + half_excl_suffix_sum(gw * w, s_w, qtot);
-        suffix += qtot;
-        if (active) {
-          dsigma = (gw * T - suf / v) * (kk * delta * M.density_scale) * (1.0f - alpha);
-          masked = w > 1e-4f;
-          if (masked) { da[0] = w * gi0; da[1] = w * gi1; }
-        }
-      }
+      float* dq = A.sv.dfeat + l4d_dfeat_off(A.sv, ray, j);     // this row in the dfeat tile (float4 per 4 features)
+      const uint32_t slot = tile_no & 1u;
+      if (tid == 0) s_heads[slot ^ 1u] = 0u;     // the previous tile's flags: read by every thread before its last barrier
+      ++tile_no;
       if (half == 0) {      // per-row values for the fragment epilogues (visible after the barrier in publish below)
-        s_dsig[row] = dsigma;
-        s_da[row] = da[0];
-        s_da[128 + row] = da[1];
-        s_mk[row] = masked ? 1.f : 0.f;
+        const float4 c = active ? *reinterpret_cast<const float4*>(dq) : make_float4(0.f, 0.f, 0.f, 0.f);   // k_bwd_composite
+        s_dsig[row] = c.x;
+        s_da[row] = c.y;
+        s_da[128 + row] = c.z;
+        s_mk[row] = c.w;
+        const uint32_t b = (__ballot_sync(0xffffffffu, c.y != 0.f) ? 1u : 0u) | (__ballot_sync(0xffffffffu, c.z != 0.f) ? 2u : 0u);
+        if ((tid & 31) == 0 && b) atomicOr(&s_heads[slot], b << (2 * (row >> 6)));
       }
       // this thread's fragment rows: m0 + frag_row() + 8h
       const int fr = m0 + frag_row();
@@ -650,27 +708,28 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
       for (int i = 0; i < 8; ++i) dgeo[i] = 0.f;
 
       L4D_PH(3);
-      // ---------------- P2: attribute heads ----------------
-      bool x_dirty = false;          // the attribute phase reuses the X buffer for its tiles
-      if (__syncthreads_or(masked ? 1 : 0)) {
-        // [geo, 1] tile, zero rows for samples outside the attribute mask: geo from the fragment, then the row fix-up
-        frag_put16_shift<-1>(g16h, g16l, m0, out);
-        __syncthreads();
-        if (half == 0) {
-          if (masked) tile_put1(g16h, g16l, row, 15, 1.0f);
-          else {
-            *reinterpret_cast<uint4*>(tile_chunk(g16h, row, 0)) = make_uint4(0u, 0u, 0u, 0u);
-            *reinterpret_cast<uint4*>(tile_chunk(g16h, row, 1)) = make_uint4(0u, 0u, 0u, 0u);
-            *reinterpret_cast<uint4*>(tile_chunk(g16l, row, 0)) = make_uint4(0u, 0u, 0u, 0u);
-            *reinterpret_cast<uint4*>(tile_chunk(g16l, row, 1)) = make_uint4(0u, 0u, 0u, 0u);
+      // ---------------- P2: attribute heads (each warpgroup on its own rows) ----------------
+      const uint32_t heads = s_heads[slot];
+      const uint32_t mine = (heads >> (2 * wg)) & 3u, theirs = (heads >> (2 * (wg ^ 1))) & 3u;
+      const bool x_dirty = heads != 0u;        // the attribute phase reuses the X buffer for its tiles
+      if (mine) {
+        // [geo, 1] tile rows of this warpgroup; zero rows for samples outside the attribute mask
+        const bool mk[2] = {s_mk[fr] != 0.f, s_mk[fr + 8] != 0.f};
+        {
+          float gv[8];
+#pragma unroll
+          for (int i = 0; i < 8; ++i) gv[i] = mk[(i >> 1) & 1] ? out[i] : 0.f;
+          frag_put16_shift<-1>(g16h, g16l, m0, gv);
+          if ((tid & 3) == 0) {
+            tile_put1(g16h, g16l, fr, 15, mk[0] ? 1.0f : 0.f);
+            tile_put1(g16h, g16l, fr + 8, 15, mk[1] ? 1.0f : 0.f);
           }
         }
-        const bool mk[2] = {s_mk[fr] != 0.f, s_mk[fr + 8] != 0.f};
 #pragma unroll 1
         for (int net = 0; net < 2; ++net) {
-          if (!__syncthreads_or(da[net] != 0.f ? 1 : 0)) continue;       // no gradient reaches this head in this tile
-          x_dirty = true;
-          publish();
+          if (!((mine >> net) & 1u)) continue;       // no gradient reaches this head on this warpgroup's rows
+          const bool pair = (theirs >> net) & 1u;    // the other warpgroup forms partials of this head's weight gradients too
+          wg_publish();
           float d[32], v[32];
           mma_rows<64>(d, m0, aG16h, aG16l, sb + L.wa1[net], 64, 2);
 #pragma unroll
@@ -694,8 +753,8 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
               const float a = l4d_sigmoid(quad_sum(o[h]));
               d_raw[h] = mk[h] ? s_da[net * 128 + fr + 8 * h] * a * (1.0f - a) : 0.f;
             }
-            // per-tile power-of-two scale of the delta tiles (|w3| <= w3max bounds the second tile too)
-            const float am = block_amax256(fmaxf(fabsf(d_raw[0]), fabsf(d_raw[1])) * s_w3max[net], s_w);
+            // power-of-two scale of this warpgroup's rows of the delta tiles (|w3| <= w3max bounds the second tile too)
+            const float am = wg_amax(fmaxf(fabsf(d_raw[0]), fabsf(d_raw[1])) * s_w3max[net], s_w);
             cs = am > 0.f ? pow2_factor(am) : 1.0f;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
@@ -710,28 +769,47 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
               v[i] = ((m2 >> i) & 1u) ? l4d_ld1(M.att_w3[net] + 8 * (i >> 2) + frag_col() + (i & 1)) * d_o[(i >> 1) & 1] : 0.f;
             frag_put<64>(t3h, t3l, 128, m0, 0, v);
           }
-          publish();
+          wg_publish();
           const float inv = 1.0f / cs;
-          // dw3^T[64 x 8] = H2^T * dO (column 0 carries dO; warpgroup 0)
-          if (wg == 0)
-            mma_tt<8>(aT2h, aT2l, aO8h, aO8l, [&](int r, int c, float x, float) {
-              if (c == 0) atomicAdd(G.att_w3[net] + r, x * inv);
-            });
-          // dW2^T[64 x 64] = H1^T * dH2 (warpgroup w: columns [32w, 32w + 32))
-          mma_tt<32>(aT1h, aT1l, aT3h + (uint32_t)wg * 4u * 2048u, aT3l + (uint32_t)wg * 4u * 2048u, [&](int r, int c, float x, float y) {
-            red2(G.att_w2t[net] + (size_t)r * 64 + 32 * wg + c, x * inv, y * inv);
-          });
+          {   // dw3^T[64 x 8] = H2^T * dO (column 0 carries dO) and dW2^T[64 x 64] = H1^T * dH2 over this warpgroup's samples
+            float p3[4], p2[32];
+            mma_tt64_issue<8>(p3, m0, aT2h, aT2l, aO8h, aO8l);
+            mma_tt64_issue<64>(p2, m0, aT1h, aT1l, aT3h, aT3l);
+            wg_wait<0>();
+            if (pair && wg == 1) {           // hand the partials to warpgroup 0
+              if (slab2_busy) pair_wait(4);
+#pragma unroll
+              for (int i = 0; i < 32; ++i) slab2[i * 128 + lt] = p2[i] * inv;
+              slab2[32 * 128 + lt] = p3[0] * inv;
+              slab2[33 * 128 + lt] = p3[2] * inv;
+              pair_arrive(3);
+              slab2_busy = true;
+            } else {
+              if (pair) pair_wait(3);
+              frag_foreach<8>(p3, [&](int r, int c, float x, float) {
+                if (c == 0) atomicAdd(G.att_w3[net] + r, pair ? x * inv + slab2[(32 + (r & 8) / 8) * 128 + lt] : x * inv);
+              });
+              int k = 0;
+              frag_foreach<64>(p2, [&](int r, int c, float x, float y) {
+                float a = x * inv, b = y * inv;
+                if (pair) { a += slab2[k * 128 + lt]; b += slab2[(k + 1) * 128 + lt]; }
+                k += 2;
+                red2(G.att_w2t[net] + (size_t)r * 64 + c, a, b);
+              });
+              if (pair) pair_arrive(4);
+            }
+          }
           // dH1[64 x 64] = dH2 * W2 on this warpgroup's rows
           mma_prop<64>(d, m0, aT3h, aT3l, 8, sb + L.wa2[net], 64);
           float inv2;      // (1 / cs) / r: cs r can pass 2^128, where 1 / (cs r) is 0 rather than a subnormal
-          {   // re-scale the propagated delta with its own amax, then dH1 * relu1 -> T2 (H2 is dead past the barrier)
+          {   // re-scale the propagated delta with its own amax, then dH1 * relu1 -> T2 (H2 is dead: its products have completed)
             float am = 0.f;
 #pragma unroll
             for (int i = 0; i < 32; ++i) {
               v[i] = ((m1 >> i) & 1u) ? d[i] : 0.f;
               am = fmaxf(am, fabsf(v[i]));
             }
-            am = block_amax256(am, s_w);
+            am = wg_amax(am, s_w);
             const float r = am > 0.f ? pow2_factor(am) : 1.0f;
             inv2 = (1.0f / cs) / r;
 #pragma unroll
@@ -739,20 +817,34 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
             frag_put<64>(t2h, t2l, 128, m0, 0, v);
           }
           L4D_PH(4);
-          publish();
-          // dW1g[64 x 16] = dH1^T * [geo,1] (warpgroup w: columns [8w, 8w + 8); column 15 is the ones column)
-          mma_tt<8>(aT2h, aT2l, aG16h + (uint32_t)wg * 2048u, aG16l + (uint32_t)wg * 2048u, [&](int r, int c, float x, float y) {
-            const int ii = 8 * wg + c;
-            atomicAdd(G.att_w1t[net] + (size_t)(L4D_ENC + ii) * 64 + r, x * inv2);
-            if (ii + 1 < 15) atomicAdd(G.att_w1t[net] + (size_t)(L4D_ENC + ii + 1) * 64 + r, y * inv2);
-            else s_csum[net * 64 + r] += y * inv2;
-          });
-          // dG[64 x 16] = dH1 * W1g on this warpgroup's rows
-          {
-            float g[8];
-            mma_prop<16>(g, m0, aT2h, aT2l, 8, sb + L.wa1[net], 64);
+          wg_publish();
+          {   // dW1g[64 x 16] = dH1^T * [geo,1] over this warpgroup's samples (column 15 is the ones column) and
+              // dG[64 x 16] = dH1 * W1g on its rows
+            float p1[8], g[8];
+            mma_tt64_issue<16>(p1, m0, aT2h, aT2l, aG16h, aG16l);
+            mma_prop_issue<16>(g, m0, aT2h, aT2l, 8, sb + L.wa1[net], 64);
+            wg_wait<0>();
 #pragma unroll
             for (int i = 0; i < 8; ++i) dgeo[i] = fmaf(g[i], inv2, dgeo[i]);
+            if (pair && wg == 1) {
+              if (slab1_busy) pair_wait(6);
+#pragma unroll
+              for (int i = 0; i < 8; ++i) slab1[i * 128 + lt] = p1[i] * inv2;
+              pair_arrive(5);
+              slab1_busy = true;
+            } else {
+              if (pair) pair_wait(5);
+              int k = 0;
+              frag_foreach<16>(p1, [&](int r, int c, float x, float y) {
+                float a = x * inv2, b = y * inv2;
+                if (pair) { a += slab1[k * 128 + lt]; b += slab1[(k + 1) * 128 + lt]; }
+                k += 2;
+                atomicAdd(G.att_w1t[net] + (size_t)(L4D_ENC + c) * 64 + r, a);
+                if (c + 1 < 15) atomicAdd(G.att_w1t[net] + (size_t)(L4D_ENC + c + 1) * 64 + r, b);
+                else s_csum[net * 64 + r] += b;
+              });
+              if (pair) pair_arrive(6);
+            }
           }
           L4D_PH(6);
         }
@@ -774,7 +866,6 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
         am = fmaxf(am, fabsf(dgeo[i]));
       }
       const float amax = block_amax256(am, s_w);
-      float* dq = A.sv.dfeat + l4d_dfeat_off(A.sv, ray, j);     // this row in the dfeat tile (float4 per 4 features)
       if (amax == 0.f) {           // nothing flows back through this tile
         if (active) for (int kq = half; kq < (int)A.sv.d_quads; kq += 2) *reinterpret_cast<float4*>(dq + (size_t)kq * 512) = make_float4(0.f, 0.f, 0.f, 0.f);
         __syncthreads();
@@ -880,6 +971,10 @@ __global__ void __launch_bounds__(256) k_bwd_dense_tc(const __grid_constant__ Sp
       if (r < L4D_ENC) atomicAdd(G.att_w1t[net] + (size_t)r * 64 + jx, s_enc[r] * cs);
       else atomicAdd(G.att_w1t[net] + (size_t)(M.attr_in_dim + (r - L4D_ENC)) * 64 + jx, cs);
     }
+  }
+  if (wg == 1) {          // warpgroup 0 has read the last partials handed to it
+    if (slab2_busy) pair_wait(4);
+    if (slab1_busy) pair_wait(6);
   }
 #ifdef L4D_PHASE_CLOCKS
   __syncthreads();

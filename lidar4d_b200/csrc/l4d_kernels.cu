@@ -1143,7 +1143,7 @@ static void fill_split(SplitArgs& A, const L4DConfig* cfg, const void* staged, c
 // Dynamic shared memory of the tensor-core kernels: the carve-up plus the 128-byte alignment of its base
 static size_t tc_dyn_smem(uint32_t bytes) { return (size_t)bytes + 128; }
 // the tensor-core dense kernels hold a 128 x sigma_in_pad fp16 hi|lo tile in shared memory; on sm_90 (227 KB per CTA)
-// the backward's carve-up (196 KB) fits the largest input a valid configuration has (176: 16 hash levels, 4 plane scales)
+// the backward's carve-up (217 KB) fits the largest input a valid configuration has (176: 16 hash levels, 4 plane scales)
 static bool use_tc_dense(const L4DConfig* cfg) {
   static int optin = 0;
   if (!optin) {
@@ -1152,6 +1152,44 @@ static bool use_tc_dense(const L4DConfig* cfg) {
     cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
   }
   return cfg->mlp_fp16 && cfg->sigma_in_pad <= 192 && tc_dyn_smem(dense_bwd_smem(cfg->sigma_in_pad).total) + 128 <= (size_t)optin;
+}
+
+// compositing backward of the tensor-core pipeline: per-sample dL/dsigma, attribute deltas and mask into quad 0 of the
+// dL/dfeature tiles, where k_bwd_dense_tc picks them up
+static int launch_bwd_composite(const SplitArgs& A, cudaStream_t st) {
+  int grid;
+  const int rc = grid_for(k_bwd_composite, 128, 0, A.n_rays, grid);
+  if (rc != L4D_OK) return rc;
+  ++g_launches; k_bwd_composite<<<grid, 128, 0, st>>>(A);
+  prof_mark(st, "k_bwd_composite");
+  return L4D_OK;
+}
+
+// k_bwd_composite alone, on the saved buffer of a training forward: afterwards feature columns 0..3 of the saved
+// dL/dfeature hold {dL/dsigma, dL/da0, dL/da1, attribute mask} of every sample
+extern "C" int l4d_composite_backward(const L4DConfig* cfg, const L4DRays* rays, void* saved, size_t saved_bytes,
+                                      const float* g_depth, const float* g_image, const float* g_wsum, const float* g_weights,
+                                      void* stream) {
+  int rc = check_config(cfg);
+  if (rc != L4D_OK) return rc;
+  rc = check_rays(rays);
+  if (rc != L4D_OK) return rc;
+  if (!saved || !g_depth || !g_image) return l4d_fail(L4D_EINVAL, "null pointer");
+  if (!use_tc_dense(cfg)) return l4d_fail(L4D_EINVAL, "l4d_composite_backward: tensor-core configurations only");
+  if (saved_bytes < saved_layout(cfg, rays->n_rays, rays->n_steps).total) return l4d_fail(L4D_ESIZE, "saved buffer too small");
+  if (rays->n_rays == 0) return L4D_OK;
+  SplitArgs A;
+  memset(&A, 0, sizeof(A));
+  A.M.near_lidar = cfg->near_lidar; A.M.far_lidar = cfg->far_lidar;
+  A.M.active_sensor = cfg->active_sensor; A.M.density_scale = cfg->density_scale;
+  A.n_rays = rays->n_rays; A.S = rays->n_steps; A.perturb = rays->perturb;
+  A.seed = rays->seed; A.ray_offset = rays->ray_offset;
+  A.g_depth = g_depth; A.g_image = g_image; A.g_wsum = g_wsum; A.g_weights = g_weights;
+  A.sv = saved_view(cfg, saved, rays->n_rays, rays->n_steps);
+  rc = launch_bwd_composite(A, (cudaStream_t)stream);
+  if (rc != L4D_OK) return rc;
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
 }
 
 extern "C" int l4d_render_forward(const L4DConfig* cfg, const void* staged, const L4DFrame* frame, const L4DRays* rays,
@@ -1312,6 +1350,8 @@ extern "C" int l4d_render_backward_ex(const L4DConfig* cfg, const void* staged, 
     const size_t P = (size_t)rays->n_rays * rays->n_steps;
     const uint32_t tiles = (uint32_t)((P + L4D_NT - 1) / L4D_NT);
     if (use_tc_dense(cfg)) {
+      rc = launch_bwd_composite(A, st);
+      if (rc != L4D_OK) return rc;
       const size_t smem = tc_dyn_smem(dense_bwd_smem(cfg->sigma_in_pad).total);
       int grid;
       rc = grid_for(k_bwd_dense_tc, 256, smem, rays->n_rays, grid);

@@ -18,7 +18,7 @@ sel = np.linspace(0, 65535, N).astype(np.int64)
 ro_t, rd_t = torch.from_numpy(ro[sel])[None].to(dev), torch.from_numpy(rd[sel])[None].to(dev)
 lib = _capi.load_library()
 buf = (ctypes.c_ulonglong * 32)()
-names = {0: "ray prologue", 1: "compositing", 2: "load_x #1", 3: "P1 mma+epilogues", 4: "P2 heads fwd, dw3/dW2, dH1",
+names = {0: "ray prologue", 1: "per-row values (k_bwd_composite)", 2: "load_x #1", 3: "P1 mma+epilogues", 4: "P2 heads fwd, dw3/dW2, dH1",
          6: "P2 dW1g, dG", 7: "P3", 8: "load_x #2", 9: "P4 dW1 (mma + flush)", 11: "P4 dX (-> dfeat)", 12: "ray epilogue"}
 for it in range(3):
     m.zero_grad(set_to_none=True)
