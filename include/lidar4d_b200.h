@@ -301,7 +301,9 @@ int    l4d_chamfer_backward(const float* xyz1, const float* xyz2, uint32_t b, ui
  * pose = DEVICE [4][4] row-major cam2world; inds = n flat pixel ids row*W+col (NULL = all H*W pixels in order, n = H*W);
  * writes rays_o[n,3], rays_d[n,3] and, if gt != NULL, gt[n,C] = image[inds,C] (image = DEVICE [H*W,C]).
  * l4d_lidar_loss replaces model/runner.py:179-213 (default criteria: L1 depth, MSE intensity / raydrop, label smoothing):
- * ACCUMULATES the summed loss into *loss (zero it first) and writes d loss / d depth [n] and d loss / d image [n,2]. */
+ * ACCUMULATES the summed loss into *loss (zero it first) and writes d loss / d depth [n] and d loss / d image [n,2].
+ * It is l4d_main_loss with the default criteria and no chamfer term (the same fixed-order sum, so the same bits on
+ * every call); n = 0 adds nothing. */
 int    l4d_lidar_rays(const float* pose, float fov_up, float fov, uint32_t H, uint32_t W, const long long* inds_or_null,
                       uint32_t n, const float* image_or_null, uint32_t C, float* rays_o, float* rays_d, float* gt_or_null,
                       void* stream);
@@ -341,6 +343,37 @@ int    l4d_los_loss(const float* weights, const float* z_vals, const float* gt3,
                     float* loss, void* work, size_t work_bytes, void* stream);
 int    l4d_los_loss_backward(const float* weights, const float* z_vals, const float* gt3, uint32_t n, uint32_t S, double eps,
                              const void* work, const float* g_loss, float* g_weights, void* stream);
+
+/* --- the main LiDAR loss of train_step (model/runner.py:193-220) and eval_step (:409-421), every criterion ----------------
+ * Inputs are fp32 device arrays: depth[n], image2[n, 2] = (ray drop, intensity), gt3[n, 3] = (raydrop m, intensity,
+ * depth).  crit_* are L4D_GRAD_* codes (main_lidar4d.py:183-188), delta the huber delta, (float)(0.2 * opt.scale) with
+ * the product in double.  Sums are taken in double in a fixed order: the same inputs give the same bits.
+ * l4d_main_loss: WRITES *loss = (a_d C_d(depth m, gt_d) + a_r C_r(r, clamp(m, s, 1 - s)) + a_i C_i(int m, gt_i)).sum()
+ *   with r = image_0, or sigmoid(image_0) for bce (BCEWithLogits then applies its own sigmoid, as the reference does);
+ *   a cos term is CosineSimilarity over all n rays, counted n times when another term is elementwise and once when all
+ *   three are cos.  With rays_d[n, 3] != NULL it adds 0.5 mean(dist1 + dist2) of the chamfer distances between
+ *   rays_d * depth m / scale and rays_d * gt_d / scale (scale > 0; ties go to the smallest index).  Writes g_depth[n]
+ *   and g_image2[n, 2] = d loss / d (depth, image) for a unit upstream gradient.  work = l4d_main_loss_work_bytes(n)
+ *   bytes when rays_d != NULL (L4D_ESIZE when smaller; it may be NULL otherwise); it begins with the two clouds,
+ *   prediction then ground truth, [n, 3] each.  1 <= n < 2^31.  One launch without the chamfer term; with it the
+ *   chamfer op's launches (l4d_chamfer_forward / _backward) and one more.
+ * l4d_main_loss_backward: g_depth = g_saved_depth * *g_loss and g_image2 = g_saved_image2 * *g_loss, the incoming
+ *   gradient read from device memory.  One launch.
+ * l4d_main_eval_loss: WRITES *loss = a_d mean C_d(depth mask, gt_d) + a_r mean C_r(r, m) + a_i mean C_i(int mask, gt_i)
+ *   over [B, H, W] images, mask = r > 0.5 (0 for NaN).  r is raydrop (B*H*W elements of dtype raydrop_dtype =
+ *   L4D_DTYPE_*, the U-Net's output) when given, else image_0, or sigmoid(image_0) for bce.  A cos term is the mean
+ *   of the per-column cosines over H, as CosineSimilarity(dim=1).  No gradient.  One launch.
+ * Null required pointers, n = 0, unknown criteria or dtypes: L4D_EINVAL. */
+size_t l4d_main_loss_work_bytes(uint32_t n);
+int    l4d_main_loss(const float* depth, const float* image2, const float* gt3, const float* rays_d_or_null, uint32_t n,
+                     uint32_t crit_d, uint32_t crit_r, uint32_t crit_i, float alpha_d, float alpha_r, float alpha_i,
+                     double smooth, float scale, float delta, float* loss, float* g_depth, float* g_image2, void* work,
+                     size_t work_bytes, void* stream);
+int    l4d_main_loss_backward(const float* g_saved_depth, const float* g_saved_image2, uint32_t n, const float* g_loss,
+                              float* g_depth, float* g_image2, void* stream);
+int    l4d_main_eval_loss(const float* depth, const float* image2, const float* gt3, const void* raydrop_or_null,
+                          uint32_t raydrop_dtype, uint32_t B, uint32_t H, uint32_t W, uint32_t crit_d, uint32_t crit_r,
+                          uint32_t crit_i, float alpha_d, float alpha_r, float alpha_i, float delta, float* loss, void* stream);
 
 /* --- exact nearest-neighbour search through a uniform grid, and the flow loss of train_step (model/runner.py:222-253) -----
  * For clouds that are searched many times (every optimiser step of the flow loss).  b = 1 only; xyz[n, 3] fp32, 1 <= n < 2^31.

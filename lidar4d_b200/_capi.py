@@ -160,6 +160,7 @@ EXPORTS = [
     "l4d_sweep_images",
     "l4d_box_mask", "l4d_bce_loss_work_bytes", "l4d_bce_loss", "l4d_bce_loss_backward",
     "l4d_composite_backward",
+    "l4d_main_loss_work_bytes", "l4d_main_loss", "l4d_main_loss_backward", "l4d_main_eval_loss",
 ]
 SWEEP_SIM, SWEEP_TEST, SWEEP_EVAL = 0, 1, 2     # L4D_SWEEP_* layouts of l4d_sweep_images
 SWEEP_F32, SWEEP_F16 = 0, 1                     # L4D_SWEEP_* ray-drop dtypes
@@ -280,6 +281,13 @@ def declare(lib, prefix: str = "l4d_", host_sim: bool = False):
         lib.l4d_bce_loss.argtypes = [V, U32, V, U32, V, V, SZ, V]
         lib.l4d_bce_loss_backward.argtypes = [V, U32, V, U32, V, V, V]
         for n in ("box_mask", "bce_loss", "bce_loss_backward"):
+            getattr(lib, f"l4d_{n}").restype = C.c_int
+        lib.l4d_main_loss_work_bytes.argtypes = [U32]
+        lib.l4d_main_loss_work_bytes.restype = SZ
+        lib.l4d_main_loss.argtypes = [V, V, V, V, U32, U32, U32, U32, F, F, F, C.c_double, F, F, V, V, V, V, SZ, V]
+        lib.l4d_main_loss_backward.argtypes = [V, V, U32, V, V, V, V]
+        lib.l4d_main_eval_loss.argtypes = [V, V, V, V, U32, U32, U32, U32, U32, U32, U32, F, F, F, F, V, V]
+        for n in ("main_loss", "main_loss_backward", "main_eval_loss"):
             getattr(lib, f"l4d_{n}").restype = C.c_int
         D, F = C.c_double, C.c_float
         for n in ("range_filter", "outlier_select", "ground_split"):

@@ -1722,13 +1722,89 @@ extern "C" int l4d_lidar_rays(const float* pose, float fov_up, float fov, uint32
   return L4D_OK;
 }
 
+// the main LiDAR loss (l4d_losses.cuh): one CTA for the criteria, then, with the chamfer term, l4d_chamfer_forward /
+// _backward on the two clouds and one CTA that adds the chamfer mean and folds its gradient into d loss / d depth
+static int main_loss_run(const float* depth, const float* image, const float* gt, const float* rays_d, uint32_t n,
+                         const uint32_t* crit, const float* alpha, double smooth, float scale, float delta, uint32_t accumulate,
+                         float* loss, float* g_depth, float* g_image, void* work, size_t work_bytes, void* stream,
+                         const char* who) {
+  if (!depth || !image || !gt || !loss || !g_depth || !g_image) return l4d_fail(L4D_EINVAL, "%s: null pointer", who);
+  if (n == 0 || n > 0x7fffffffu) return l4d_fail(L4D_EINVAL, "%s: n must be in [1, 2^31)", who);
+  for (int k = 0; k < L4D_MT_N; ++k)
+    if (crit[k] > L4D_GRAD_COS) return l4d_fail(L4D_EINVAL, "%s: unknown criterion", who);
+  if (rays_d && !(scale > 0.f && isfinite(scale))) return l4d_fail(L4D_EINVAL, "%s: the chamfer term needs scale > 0", who);
+  const L4DMainLayout L = l4d_main_layout(n);
+  if (rays_d && !work) return l4d_fail(L4D_EINVAL, "%s: null work buffer", who);
+  if (rays_d && work_bytes < L.total) return l4d_fail(L4D_ESIZE, "%s: work buffer too small", who);
+  const L4DMainArgs a = l4d_main_args(n, crit, alpha, smooth, scale, delta);
+  cudaStream_t st = (cudaStream_t)stream;
+  L4DMainPtrs P = {};
+  char* w = static_cast<char*>(work);
+  if (rays_d) {
+    P.pred = (float*)(w + L.pred); P.gtc = (float*)(w + L.gtc); P.d1 = (float*)(w + L.d1); P.d2 = (float*)(w + L.d2);
+    P.gdist = (float*)(w + L.gdist); P.gx1 = (float*)(w + L.gx1); P.gx2 = (float*)(w + L.gx2); P.crit_sum = (double*)(w + L.hdr);
+  }
+  ++g_launches;
+  k_main_loss<<<1, L4D_MAIN_THREADS, 0, st>>>(depth, image, gt, rays_d, n, a, P, accumulate, loss, g_depth, g_image);
+  L4D_CUDA(cudaGetLastError());
+  if (!rays_d) return L4D_OK;
+  int32_t* i1 = (int32_t*)(w + L.i1);
+  int32_t* i2 = (int32_t*)(w + L.i2);
+  if (int rc = l4d_chamfer_forward(P.pred, P.gtc, 1, n, n, P.d1, P.d2, i1, i2, w + L.keys, 2 * (size_t)n * 8, stream)) return rc;
+  if (int rc = l4d_chamfer_backward(P.pred, P.gtc, 1, n, n, P.gdist, P.gdist + n, i1, i2, P.gx1, P.gx2, stream)) return rc;
+  ++g_launches;
+  k_main_finish<<<1, L4D_MAIN_THREADS, 0, st>>>(gt, rays_d, n, a, P, accumulate, loss, g_depth);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
 extern "C" int l4d_lidar_loss(const float* depth, const float* image, const float* gt, uint32_t n, float alpha_d, float alpha_r,
                               float alpha_i, float smooth, float* loss, float* g_depth, float* g_image, void* stream) {
-  if (!depth || !image || !gt || !loss || !g_depth || !g_image) return l4d_fail(L4D_EINVAL, "l4d_lidar_loss: null pointer");
-  if (n == 0) return L4D_OK;
-  int grid = nblk(n);
+  if (n == 0 && depth && image && gt && loss && g_depth && g_image) return L4D_OK;
+  const uint32_t crit[L4D_MT_N] = {L4D_GRAD_L1, L4D_GRAD_MSE, L4D_GRAD_MSE};
+  const float alpha[L4D_MT_N] = {alpha_d, alpha_r, alpha_i};
+  return main_loss_run(depth, image, gt, nullptr, n, crit, alpha, smooth, 0.f, 0.f, 1, loss, g_depth, g_image, nullptr, 0,
+                       stream, "l4d_lidar_loss");
+}
+
+extern "C" size_t l4d_main_loss_work_bytes(uint32_t n) { return l4d_main_layout(n).total; }
+
+extern "C" int l4d_main_loss(const float* depth, const float* image, const float* gt, const float* rays_d, uint32_t n,
+                             uint32_t crit_d, uint32_t crit_r, uint32_t crit_i, float alpha_d, float alpha_r, float alpha_i,
+                             double smooth, float scale, float delta, float* loss, float* g_depth, float* g_image, void* work,
+                             size_t work_bytes, void* stream) {
+  const uint32_t crit[L4D_MT_N] = {crit_d, crit_r, crit_i};
+  const float alpha[L4D_MT_N] = {alpha_d, alpha_r, alpha_i};
+  return main_loss_run(depth, image, gt, rays_d, n, crit, alpha, smooth, scale, delta, 0, loss, g_depth, g_image, work,
+                       work_bytes, stream, "l4d_main_loss");
+}
+
+extern "C" int l4d_main_loss_backward(const float* g_saved_depth, const float* g_saved_image, uint32_t n, const float* g_loss,
+                                      float* g_depth, float* g_image, void* stream) {
+  if (!g_saved_depth || !g_saved_image || !g_loss || !g_depth || !g_image)
+    return l4d_fail(L4D_EINVAL, "l4d_main_loss_backward: null pointer");
+  if (n == 0 || n > 0x7fffffffu) return l4d_fail(L4D_EINVAL, "l4d_main_loss_backward: n must be in [1, 2^31)");
+  int grid = nblk(3 * (size_t)n);
   if (grid > 4 * sm_count()) grid = 4 * sm_count();
-  ++g_launches; k_lidar_loss<<<grid, 256, 0, (cudaStream_t)stream>>>(depth, image, gt, n, alpha_d, alpha_r, alpha_i, smooth, loss, g_depth, g_image);
+  ++g_launches; k_main_scale<<<grid, 256, 0, (cudaStream_t)stream>>>(g_saved_depth, g_saved_image, g_loss, n, g_depth, g_image);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+extern "C" int l4d_main_eval_loss(const float* depth, const float* image, const float* gt, const void* raydrop, uint32_t raydrop_dtype,
+                                  uint32_t B, uint32_t H, uint32_t W, uint32_t crit_d, uint32_t crit_r, uint32_t crit_i,
+                                  float alpha_d, float alpha_r, float alpha_i, float delta, float* loss, void* stream) {
+  if (!depth || !image || !gt || !loss) return l4d_fail(L4D_EINVAL, "l4d_main_eval_loss: null pointer");
+  const unsigned long long n = (unsigned long long)B * H * W;
+  if (n == 0 || n > 0x7fffffffull) return l4d_fail(L4D_EINVAL, "l4d_main_eval_loss: B*H*W must be in [1, 2^31)");
+  if (crit_d > L4D_GRAD_COS || crit_r > L4D_GRAD_COS || crit_i > L4D_GRAD_COS)
+    return l4d_fail(L4D_EINVAL, "l4d_main_eval_loss: unknown criterion");
+  if (raydrop && raydrop_dtype > L4D_DTYPE_BF16) return l4d_fail(L4D_EINVAL, "l4d_main_eval_loss: unknown ray-drop dtype");
+  const uint32_t crit[L4D_MT_N] = {crit_d, crit_r, crit_i};
+  const float alpha[L4D_MT_N] = {alpha_d, alpha_r, alpha_i};
+  const L4DMainArgs a = l4d_main_args((uint32_t)n, crit, alpha, 0.0, 0.f, delta);
+  ++g_launches;
+  k_main_eval<<<1, L4D_MAIN_THREADS, 0, (cudaStream_t)stream>>>(depth, image, gt, raydrop, raydrop_dtype, B, H, W, a, loss);
   L4D_CUDA(cudaGetLastError());
   return L4D_OK;
 }

@@ -1,9 +1,7 @@
-// l4d_rays.cuh - SURVEY.md 8(f) #2: the two thin layers around the render kernels, one launch each instead of the
-// reference's chains of elementwise torch ops:
+// l4d_rays.cuh - SURVEY.md 8(f) #2: the thin layer in front of the render kernels, one launch instead of the
+// reference's chain of elementwise torch ops (the main loss behind them is in l4d_losses.cuh):
 //   k_lidar_rays   data/base_dataset.py:15-102 get_lidar_rays (pixel -> azimuth / elevation -> direction @ R^T, origin)
 //                  + the ground-truth gather of data/kitti360_dataset.py:170-178 (images_lidar[inds])
-//   k_lidar_loss   model/runner.py:179-213 main loss (label-smoothed raydrop MSE, masked L1 depth, masked MSE intensity),
-//                  value AND gradient with respect to the render outputs in one pass
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -34,32 +32,4 @@ __global__ void __launch_bounds__(256) k_lidar_rays(const float* __restrict__ po
   }
   if (gt && image)
     for (uint32_t c = 0; c < C; ++c) gt[(size_t)r * C + c] = image[(size_t)pix * C + c];
-}
-
-// loss += sum_r [ a_d |depth*m - gt_d*m| + a_r (raydrop - clamp(m, s, 1-s))^2 + a_i (inten*m - gt_i*m)^2 ],  m = gt raydrop
-// g_depth / g_image = d loss / d (depth, image)
-__global__ void __launch_bounds__(256) k_lidar_loss(const float* __restrict__ depth, const float* __restrict__ image,
-                                                    const float* __restrict__ gt, uint32_t n, float a_d, float a_r, float a_i, float smooth,
-                                                    float* __restrict__ loss, float* __restrict__ g_depth, float* __restrict__ g_image) {
-  __shared__ float s_w[8];
-  float acc = 0.f;
-  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n; r += gridDim.x * blockDim.x) {
-    const float m = gt[3 * (size_t)r], gi = gt[3 * (size_t)r + 1] * m, gd = gt[3 * (size_t)r + 2] * m;
-    const float pr = image[2 * (size_t)r], pi = image[2 * (size_t)r + 1] * m, pd = depth[r] * m;
-    const float ms = fminf(fmaxf(m, smooth), 1.0f - smooth);
-    const float ed = pd - gd, er = pr - ms, ei = pi - gi;
-    acc += a_d * fabsf(ed) + a_r * er * er + a_i * ei * ei;
-    g_depth[r] = a_d * (ed > 0.f ? 1.f : (ed < 0.f ? -1.f : 0.f)) * m;
-    g_image[2 * (size_t)r] = 2.0f * a_r * er;
-    g_image[2 * (size_t)r + 1] = 2.0f * a_i * ei * m;
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float t = 0.f;
-    for (int w = 0; w < 8; ++w) t += s_w[w];
-    atomicAdd(loss, t);
-  }
 }

@@ -1,14 +1,17 @@
-"""Main LiDAR loss of the reference's train_step (model/runner.py:179-213) as ONE CUDA launch that returns the summed
-loss and, in the same pass, its gradient with respect to the render outputs (SURVEY.md 8(f) #2).
+"""The losses of the reference's train_step and eval_step as CUDA ops, each backward one launch that reads the incoming
+gradient from device memory (a GradScaler-scaled backward needs no host sync).
 
-    loss = lidar_main_loss(out["depth_lidar"], out["image_lidar"], gt, alpha_d=opt.alpha_d, alpha_r=opt.alpha_r,
-                           alpha_i=opt.alpha_i, smooth=opt.smooth_factor)
+The main loss and the chamfer term at the top of train_step (model/runner.py:193-220), for any criteria of the CLI:
 
-equals  (alpha_d*L1(depth*m, gt_d*m) + alpha_r*MSE(raydrop, clamp(m, s, 1-s)) + alpha_i*MSE(intensity*m, gt_i*m)).sum()
-with m = gt[..., 0] (ray-drop mask), gt_i = gt[..., 1], gt_d = gt[..., 2] - the default criteria of main_lidar4d.py:63-66.
+    loss = lidar_main_loss(out["depth_lidar"], out["image_lidar"], gt, opt.alpha_d, opt.alpha_r, opt.alpha_i,
+                           opt.smooth_factor, depth_loss=opt.depth_loss, raydrop_loss=opt.raydrop_loss,
+                           intensity_loss=opt.intensity_loss, scale=opt.scale, rays_d=rays_d_lidar)
 
-The rest of train_step (model/runner.py:255-369), each a CUDA op whose backward is one launch that reads the incoming
-gradient from device memory (a GradScaler-scaled backward needs no host sync):
+and eval_step's loss (:409-421), forward only:
+
+    loss = lidar_eval_loss(depth, image, gt, raydrop=unet_out_or_None, alpha_d=..., depth_loss=..., scale=opt.scale)
+
+The rest of train_step (model/runner.py:255-369):
 
     loss = loss + line_of_sight_loss(out["weights"], out["z_vals"], gt, eps)        # --urf_loss
     loss = loss + lidar_patch_loss(out["depth_lidar"], gt, **vars(opt))             # patch batches
@@ -26,11 +29,33 @@ import torch
 from . import _capi
 
 
+GRAD_CRITERIA = {"l1": 0, "mse": 1, "huber": 2, "bce": 3, "cos": 4}      # L4D_GRAD_* (main_lidar4d.py:183-188)
+_SOBEL, _GRAD, _GRAD_NORM, _SPATIAL, _TV = 1, 2, 4, 8, 16                # L4D_PATCH_*
+
+
+def _stream(t):
+    return torch.cuda.current_stream(t.device).cuda_stream
+
+
+def _criterion(name, slot):
+    if name not in GRAD_CRITERIA:
+        raise ValueError(f"{slot} must be one of {sorted(GRAD_CRITERIA)}, got {name!r}")
+    return GRAD_CRITERIA[name]
+
+
+def _huber_delta(crits, scale, who):
+    """main_lidar4d.py:187: HuberLoss(delta=0.2 * opt.scale), the product in double (rounded to fp32 by ATen's kernel and
+    by the C-ABI's float argument alike)."""
+    if GRAD_CRITERIA["huber"] in crits:
+        if scale is None:
+            raise ValueError(f"{who}: the huber criterion needs scale (its delta is 0.2 * scale)")
+        return 0.2 * float(scale)
+    return 0.0
+
+
 class _MainLoss(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, depth, image, gt, alpha_d, alpha_r, alpha_i, smooth):
-        if not depth.is_cuda:
-            raise RuntimeError("lidar_main_loss runs on CUDA only (no CPU fallback)")
+    def forward(ctx, depth, image, gt, rays_d, crits, alphas, smooth, scale, delta):
         lib = _capi.load_library()
         n = depth.numel()
         d = depth.detach().contiguous().view(-1).float()
@@ -38,34 +63,105 @@ class _MainLoss(torch.autograd.Function):
         g = gt.detach().contiguous().view(-1, 3).float()
         if im.shape[0] != n or g.shape[0] != n:
             raise ValueError("depth [.., N], image [.., N, 2] and gt [.., N, 3] must describe the same rays")
-        loss = torch.zeros((), device=d.device)
+        rd, work = None, None
+        if rays_d is not None:
+            rd = rays_d.detach().contiguous().view(-1, 3).float()
+            if rd.shape[0] != n:
+                raise ValueError("rays_d [.., N, 3] must describe the same rays as depth")
+            work = torch.empty(lib.l4d_main_loss_work_bytes(n), dtype=torch.uint8, device=d.device)
+        loss = torch.empty((), device=d.device)
         gd = torch.empty_like(d)
         gi = torch.empty_like(im)
         with torch.cuda.device(d.device):
-            rc = lib.l4d_lidar_loss(d.data_ptr(), im.data_ptr(), g.data_ptr(), n, float(alpha_d), float(alpha_r), float(alpha_i),
-                                    float(smooth), loss.data_ptr(), gd.data_ptr(), gi.data_ptr(),
-                                    torch.cuda.current_stream(d.device).cuda_stream)
-        _capi.check(lib, rc, "l4d_lidar_loss")
+            rc = lib.l4d_main_loss(d.data_ptr(), im.data_ptr(), g.data_ptr(), None if rd is None else rd.data_ptr(), n,
+                                   *crits, *(float(a) for a in alphas), float(smooth), float(scale or 0.0), float(delta),
+                                   loss.data_ptr(), gd.data_ptr(), gi.data_ptr(), None if work is None else work.data_ptr(),
+                                   0 if work is None else work.numel(), _stream(d))
+        _capi.check(lib, rc, "l4d_main_loss")
         ctx.save_for_backward(gd, gi)
         ctx.shapes = (depth.shape, image.shape)
         return loss
 
     @staticmethod
-    def backward(ctx, g):
+    def backward(ctx, gl):
         gd, gi = ctx.saved_tensors
-        return (gd * g).view(ctx.shapes[0]), (gi * g).view(ctx.shapes[1]), None, None, None, None, None
+        lib = _capi.load_library()
+        gl = gl.detach().float().contiguous()
+        od, oi = torch.empty_like(gd), torch.empty_like(gi)
+        with torch.cuda.device(gd.device):
+            rc = lib.l4d_main_loss_backward(gd.data_ptr(), gi.data_ptr(), gd.numel(), gl.data_ptr(), od.data_ptr(),
+                                            oi.data_ptr(), _stream(gd))
+        _capi.check(lib, rc, "l4d_main_loss_backward")
+        return (od.view(ctx.shapes[0]), oi.view(ctx.shapes[1])) + (None,) * 7
 
 
-def lidar_main_loss(depth, image, gt, alpha_d=1.0, alpha_r=0.01, alpha_i=0.1, smooth=0.2):
-    return _MainLoss.apply(depth, image, gt, alpha_d, alpha_r, alpha_i, smooth)
+def lidar_main_loss(depth, image, gt, alpha_d=1.0, alpha_r=0.01, alpha_i=0.1, smooth=0.2, *, depth_loss="l1",
+                    raydrop_loss="mse", intensity_loss="mse", scale=None, rays_d=None):
+    """model/runner.py:193-220 as a device scalar, differentiable in depth and image:
+
+        (alpha_d C_d(depth m, gt_d) + alpha_r C_r(r, clamp(m, s, 1 - s)) + alpha_i C_i(image_1 m, gt_i)).sum()
+        + 0.5 * mean(dist1 + dist2)      (only when rays_d is given)
+
+    with m = gt[..., 0], gt_i = gt[..., 1] m, gt_d = gt[..., 2] m, r = image[..., 0] (its sigmoid for raydrop_loss="bce",
+    which BCEWithLogits then applies again, as in the reference), C_* the criteria of main_lidar4d.py:183-188 by name
+    (l1, mse, huber, bce, cos), and dist1 / dist2 the chamfer distances between rays_d * depth m / scale and
+    rays_d * gt_d / scale.  A cos criterion is CosineSimilarity over all N rays; it counts N times when another term is
+    elementwise and once when all three are cos, as the reference's broadcast does.  depth [.., N], image [.., N, 2],
+    gt [.., N, 3], rays_d [.., N, 3].  rays_d and huber need scale.  Sums are in double in a fixed order: the same
+    inputs give the same bits.  No host read, forward or backward."""
+    crits = (_criterion(depth_loss, "depth_loss"), _criterion(raydrop_loss, "raydrop_loss"),
+             _criterion(intensity_loss, "intensity_loss"))
+    if rays_d is not None and scale is None:
+        raise ValueError("lidar_main_loss: the chamfer term (rays_d) needs scale")
+    delta = _huber_delta(crits, scale, "lidar_main_loss")
+    if not (depth.is_cuda and image.is_cuda and gt.is_cuda and (rays_d is None or rays_d.is_cuda)):
+        raise RuntimeError("lidar_main_loss runs on CUDA only (no CPU fallback)")
+    if depth.numel() == 0:
+        raise ValueError("lidar_main_loss of an empty batch")
+    return _MainLoss.apply(depth, image, gt, rays_d, crits, (alpha_d, alpha_r, alpha_i), smooth, scale, delta)
 
 
-GRAD_CRITERIA = {"l1": 0, "mse": 1, "huber": 2, "bce": 3, "cos": 4}      # L4D_GRAD_* (main_lidar4d.py:183-188)
-_SOBEL, _GRAD, _GRAD_NORM, _SPATIAL, _TV = 1, 2, 4, 8, 16                # L4D_PATCH_*
+def lidar_eval_loss(depth, image, gt, raydrop=None, *, alpha_d=1.0, alpha_r=0.01, alpha_i=0.1, depth_loss="l1",
+                    raydrop_loss="mse", intensity_loss="mse", scale=None):
+    """model/runner.py:409-421, eval_step's loss, as a float32 device scalar (no host read, no gradient):
 
+        alpha_d mean C_d(depth mask, gt_d) + alpha_r mean C_r(r, m) + alpha_i mean C_i(image_1 mask, gt_i)
 
-def _stream(t):
-    return torch.cuda.current_stream(t.device).cuda_stream
+    over gt [B, H, W, 3] (depth and image hold B*H*W and B*H*W*2 values), with mask = r > 0.5 (0 for NaN) and r the
+    ray-drop prediction: `raydrop` (the U-Net's output when refining: float32, float16 or bfloat16, B*H*W values) if
+    given, else image[..., 0], or its sigmoid for raydrop_loss="bce".  No label smoothing.  A cos criterion is the mean
+    of the per-column cosines over H, as CosineSimilarity(dim=1) gives them.  huber needs scale."""
+    crits = (_criterion(depth_loss, "depth_loss"), _criterion(raydrop_loss, "raydrop_loss"),
+             _criterion(intensity_loss, "intensity_loss"))
+    delta = _huber_delta(crits, scale, "lidar_eval_loss")
+    if not (depth.is_cuda and image.is_cuda and gt.is_cuda and (raydrop is None or raydrop.is_cuda)):
+        raise RuntimeError("lidar_eval_loss runs on CUDA only (no CPU fallback)")
+    if gt.dim() != 4 or gt.shape[-1] != 3:
+        raise ValueError("gt must be [B, H, W, 3]")
+    B, H, W = (int(x) for x in gt.shape[:3])
+    n = B * H * W
+    if depth.numel() != n or image.numel() != 2 * n:
+        raise ValueError("depth and image must hold B*H*W and B*H*W*2 values for gt [B, H, W, 3]")
+    if n == 0:
+        raise ValueError("lidar_eval_loss of an empty image")
+    lib = _capi.load_library()
+    d = depth.detach().contiguous().view(-1).float()
+    im = image.detach().contiguous().view(-1, 2).float()
+    g = gt.detach().contiguous().view(-1, 3).float()
+    r, dt = None, 0
+    if raydrop is not None:
+        if raydrop.dtype not in _BCE_DTYPES:
+            raise ValueError(f"raydrop must be float32, float16 or bfloat16, got {raydrop.dtype}")
+        if raydrop.numel() != n:
+            raise ValueError("raydrop must hold B*H*W values")
+        r, dt = raydrop.detach().contiguous(), _BCE_DTYPES[raydrop.dtype]
+    loss = torch.empty((), device=d.device)
+    with torch.cuda.device(d.device):
+        rc = lib.l4d_main_eval_loss(d.data_ptr(), im.data_ptr(), g.data_ptr(), None if r is None else r.data_ptr(), dt,
+                                    B, H, W, *crits, float(alpha_d), float(alpha_r), float(alpha_i), float(delta),
+                                    loss.data_ptr(), _stream(d))
+    _capi.check(lib, rc, "l4d_main_eval_loss")
+    return loss
 
 
 class _PatchLoss(torch.autograd.Function):
