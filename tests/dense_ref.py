@@ -43,6 +43,16 @@ rounding count times 2^-149 where an operand is non-zero.  Float atomics on glob
 results to zero, so each atomic of a weight gradient may move it by up to 2^-126: up to four per entry and tile
 (tile_outer_accum splits a tile's samples over up to four warps) and one for the per-ray sums.
 
+The point kernels (csrc/l4d_points.cuh, density_point_reference / attribute_point_reference / flow_reference(points=True))
+reduce differently, and their rounding depth per entry is 4 T_e + min(128, N_e) + C_SUM (POINT_TILE_ROUNDINGS = 4):
+  * tile_outer_accum over NT = 128 points and 4 warps: a product of K <= 16 rows gives each warp 32 points (an fma chain
+    of <= 32) and issues 4 atomics per entry and tile, so depth <= 32 + 4 T_e; K = 24: <= 64 + 2 T_e; K = 64: <= 128 + T_e.
+    With 2 T_e the first case is not covered once T_e > 56, hence 4 T_e here.
+  * dW3 of the attribute nets: tile_colsum (a chain of <= 128) and one atomicAdd per tile: <= min(128, N_e) + T_e.
+  * the 9 ones rows of the attribute nets: tile_colsum (<= 128), one add per tile into the thread's csum over the CTA's
+    grid-stride loop, one atomicAdd per CTA: <= min(128, N_e) + 2 T_e.
+The flush of subnormals stays ATOMICS_PER_TILE per tile (4 warp atomics + 1 per-CTA or per-tile colsum atomic).
+
 Tensor-core mode adds, for every delta tile the kernels scale by a power of two and split into fp16 hi + lo, the
 resolution of that tile: an entry is held to ~2^-30 of the tile's largest entry; the bound takes TC_RES = 2^-20 of it (the
 same slack as tests/test_gpu_compositing.py).  The tiles are the dense kernels' 128-sample tiles of a ray and the flow
@@ -72,6 +82,7 @@ ATOMICS_PER_TILE = 5.0           # tile_outer_accum splits a tile over up to 4 w
 C_LAYER = 8.0
 C_SUM = 16.0
 TC_RES = 2.0 ** -20
+POINT_TILE_ROUNDINGS = 4.0      # the point kernels' rounding depth per contributing tile (module docstring)
 CHUNK = 1 << 17                  # samples per pass (whole rays; keeps the float64 temporaries at a few hundred MB)
 TILE = 128
 ENC = 72                         # 3 dims x 12 frequencies x (sin, cos)
@@ -200,7 +211,8 @@ class _Grad:
     """One weight gradient Σ_p d_p ⊗ x_p: value, Σ of the products' magnitudes, propagated input error, and per entry the number of tiles
     and of samples that contribute to it (a tile without a contribution adds an exact 0)."""
 
-    def __init__(self, shape, dev):
+    def __init__(self, shape, dev, per_tile: float = 2.0):
+        self.per_tile = per_tile
         self.v = torch.zeros(shape, dtype=torch.float64, device=dev)
         self.a = torch.zeros_like(self.v)
         self.e = torch.zeros_like(self.v)
@@ -221,8 +233,9 @@ class _Grad:
 
     def result(self):
         """(value, bound): the per-entry rounding depth is at most 128 within a tile, one per contributing tile, and as
-        many again for the per-ray sums of the attribute nets' direction and ones rows."""
-        n = 2.0 * self.n_tiles + self.n_samples.clamp(max=TILE) + C_SUM
+        many again for the per-ray sums of the attribute nets' direction and ones rows (per_tile = 2); the point kernels'
+        depth is derived in the module docstring (per_tile = POINT_TILE_ROUNDINGS)."""
+        n = self.per_tile * self.n_tiles + self.n_samples.clamp(max=TILE) + C_SUM
         return self.v, self.e + _round(self.a, n) + ATOMICS_PER_TILE * FTZ * self.n_tiles
 
 
@@ -241,6 +254,94 @@ def compositing_inputs(ref: dict, U: dict, live: torch.Tensor, weight_bound: tor
     dattr_e = dattr_e + EPS32 * dattr.abs()
     return dict(dsig=ref["dsigma"].reshape(-1), dsig_e=dsigma_bound.reshape(-1),
                 dattr=dattr, dattr_e=dattr_e)
+
+
+def _sigma_forward(W: dict, x: torch.Tensor, ip: int) -> dict:
+    """Forward of the sigma MLP from exact inputs x [c, K]: the padded input, the hidden layer with its ReLU decisions,
+    the output o, σ with its bound and geo."""
+    c, K = x.shape
+    xt = exact(torch.cat([x.double(), torch.ones(c, ip - K, dtype=torch.float64, device=x.device)], 1))
+    h, on1, amb1 = _relu(_lin(xt, W["s1"], ip))
+    o = _lin(h, W["s2"], 64)
+    sig = o.v[:, 0].exp()
+    sig_b = sig * torch.expm1(o.e[:, 0]) + 3.0 * EPS32 * sig * o.e[:, 0].exp() + TINY
+    return dict(xt=xt, h=h, on1=on1, amb1=amb1, o=o, sig=sig, sig_b=sig_b, geo=V(o.v[:, 1:], o.e[:, 1:]))
+
+
+def _sigma_backward(W: dict, K: int, f: dict, ds: torch.Tensor, dse: torch.Tensor, dgeo: V, tid: torch.Tensor, tc: bool,
+                    tiles, gS1: _Grad, gS2: _Grad):
+    """Backward of the sigma MLP from dL/dσ (ds, its bound dse) and dL/dgeo; adds the weight gradients and returns
+    (dL/dX, largest log2(sc r) of the launch's tensor-core delta tiles).  tiles(x): per sample, the largest x of its tile."""
+    eo = f["o"].v[:, 0].clamp(-15.0, 15.0).exp()
+    d0 = V((ds * eo)[:, None],
+           (dse * eo + ds.abs() * eo * torch.expm1(f["o"].e[:, 0]) + _round((ds * eo).abs(), 3.0))[:, None])
+    do = V(torch.cat([d0.v, dgeo.v], 1), torch.cat([d0.e, dgeo.e], 1))
+    max_log2_scale = 0.0
+    if tc:
+        do = _rescale(do, tiles(_row_amax(do)))
+        lsc = pow2_log2(tiles(do.v.abs().amax(1)))
+    gS2.add(do, f["h"], tid)
+    dh = _back(do, W["s2"], 16, f["on1"], f["amb1"])
+    if tc:              # sc r of the sigma backward's two delta tiles, from the reference's tile maxima
+        lr = pow2_log2(tiles(dh.v.abs().amax(1)) * torch.exp2(lsc))
+        live_t = (lsc > 0) & (lr > 0)
+        if bool(live_t.any()):
+            max_log2_scale = float((lsc + lr)[live_t].max())
+        dh = _rescale(dh, tiles(_row_amax(dh)))
+    gS1.add(dh, f["xt"], tid)
+    return _back(dh, W["s1"][:, :K], 64), max_log2_scale
+
+
+def _attr_stage(W: dict, enc: torch.Tensor, enc_e: torch.Tensor, geo: V, lv: torch.Tensor, dattr: torch.Tensor,
+                dattr_e: torch.Tensor, tid: torch.Tensor, tc: bool, tiles, gA1: list, gA2: list, gA3: list):
+    """Both attribute nets, forward and backward, on c samples: enc, enc_e [c, 72] (direction encoding per sample), geo,
+    lv [c] bool (the mask), dattr, dattr_e [2, c] (dL/dattr, zero outside the mask, and its bound).  Adds the weight
+    gradients; returns (attr [2, c], its bound, dL/dgeo, samples with an ambiguous unit)."""
+    c = enc.shape[0]
+    dev = enc.device
+    m = lv.double()[:, None]
+    ones9 = torch.ones(c, W["a1_0"].shape[1] - ENC - GEO, dtype=torch.float64, device=dev)
+    a_in = V(torch.cat([enc, geo.v, ones9], 1) * m, torch.cat([enc_e, geo.e, torch.zeros_like(ones9)], 1) * m)
+    amb_attr = torch.zeros_like(lv)
+    attr_v, attr_b, dgeo = [], [], None
+    for net in range(2):
+        h1, on_a1, amb_a1 = _relu(_lin(a_in, W[f"a1_{net}"], a_in.v.shape[1]))
+        h2, on_a2, amb_a2 = _relu(_lin(h1, W[f"a2_{net}"], 64))
+        lg = _lin(h2, W[f"a3_{net}"][:1], 64)
+        s = torch.sigmoid(lg.v[:, 0])
+        sb = s * (1 - s) * lg.e[:, 0] * lg.e[:, 0].exp() + 8.0 * EPS32 * s
+        attr_v.append(s * m[:, 0])
+        attr_b.append(sb * m[:, 0])
+        amb_attr = amb_attr | (lv & (amb_a1.any(1) | amb_a2.any(1)))
+        # backward
+        da, dae = dattr[net], dattr_e[net]
+        q = s * (1 - s)
+        dl = V((da * q)[:, None],
+               (q * dae + da.abs() * ((1 - 2 * s).abs() * sb + sb * sb) + _round((da * q).abs(), 4.0))[:, None])
+        w3 = W[f"a3_{net}"][0]
+        if tc:          # dO8 and T3 tiles: scaled by cs from amax(|dl|) max(1, max|w3|)
+            am = tiles(_row_amax(dl)) * max(1.0, float(w3.abs().max()))
+            dl = _rescale(dl, am)
+        gA3[net].add(dl, h2, tid)
+        d2 = V(dl.v * w3, dl.e * w3.abs() + _round(dl.mag() * w3.abs(), 1.0))
+        if tc:
+            d2 = _rescale(d2, am)
+        d2 = _mask(d2, on_a2, amb_a2)
+        gA2[net].add(d2, h1, tid)
+        d1 = _back(d2, W[f"a2_{net}"], 64, on_a1, amb_a1)
+        if tc:
+            d1 = _rescale(d1, tiles(_row_amax(d1)))
+        gA1[net].add(d1, a_in, tid)
+        g = _back(d1, W[f"a1_{net}"][:, ENC:ENC + GEO], 64)
+        dgeo = g if dgeo is None else V(dgeo.v + g.v, dgeo.e + g.e + _round(dgeo.mag() + g.mag(), 1.0))
+    return torch.stack(attr_v), torch.stack(attr_b), dgeo, amb_attr
+
+
+def _head_results(gA1: list, gA2: list, gA3: list, out: dict, dev):
+    for net, name in enumerate(HEADS):
+        parts = [gA1[net].result(), gA2[net].result(), gA3[net].result()]
+        z = torch.zeros(15 * 64, dtype=torch.float64, device=dev)         # W3 rows 1..15: no contribution
+        out[name] = (torch.cat([p[0].reshape(-1) for p in parts] + [z]), torch.cat([p[1].reshape(-1) for p in parts] + [z]))
 
 
 def dense_reference(cfg, W: dict, X: torch.Tensor, n_rays: int, S: int, enc: torch.Tensor, enc_e: torch.Tensor,
@@ -266,107 +367,116 @@ def dense_reference(cfg, W: dict, X: torch.Tensor, n_rays: int, S: int, enc: tor
     rays_per = max(1, chunk // S)
     n_amb = n_amb_attr = 0
     max_log2_scale = 0.0
+    tiles = lambda v: _tiles_dense(v, S)
     for r0 in range(0, n_rays, rays_per):
         r1 = min(n_rays, r0 + rays_per)
         p0, p1 = r0 * S, r1 * S
         c = p1 - p0
-        x = X[p0:p1].double()
         j = torch.arange(c, device=dev)
         tid = (j // S) * ((S + TILE - 1) // TILE) + (j % S) // TILE
-        xt = exact(torch.cat([x, torch.ones(c, ip - K, dtype=torch.float64, device=dev)], 1))
-        # ---- forward ----
-        h, on1, amb1 = _relu(_lin(xt, W["s1"], ip))
-        o = _lin(h, W["s2"], 64)
-        sig = o.v[:, 0].exp()
-        sig_b = sig * torch.expm1(o.e[:, 0]) + 3.0 * EPS32 * sig * o.e[:, 0].exp() + TINY
-        geo = V(o.v[:, 1:], o.e[:, 1:])
+        f = _sigma_forward(W, X[p0:p1], ip)
         lv = live[p0:p1].to(dev)
-        m = lv.double()[:, None]
-        e_r = enc[r0:r1].repeat_interleave(S, 0)
-        ee_r = enc_e[r0:r1].repeat_interleave(S, 0)
-        ones9 = torch.ones(c, ap - ENC - GEO, dtype=torch.float64, device=dev)
-        a_in = V(torch.cat([e_r, geo.v, ones9], 1) * m, torch.cat([ee_r, geo.e, torch.zeros_like(ones9)], 1) * m)
-        amb, amb_attr = amb1.any(1), torch.zeros_like(lv)
-        attr_v, attr_b, heads = [], [], []
-        for net in range(2):
-            h1, on_a1, amb_a1 = _relu(_lin(a_in, W[f"a1_{net}"], ap))
-            h2, on_a2, amb_a2 = _relu(_lin(h1, W[f"a2_{net}"], 64))
-            lg = _lin(h2, W[f"a3_{net}"][:1], 64)
-            s = torch.sigmoid(lg.v[:, 0])
-            sb = s * (1 - s) * lg.e[:, 0] * lg.e[:, 0].exp() + 8.0 * EPS32 * s
-            attr_v.append(s * m[:, 0])
-            attr_b.append(sb * m[:, 0])
-            amb_attr = amb_attr | (lv & (amb_a1.any(1) | amb_a2.any(1)))
-            heads.append((h1, on_a1, amb_a1, h2, on_a2, amb_a2, s, sb))
-        n_amb += int(amb.sum())
+        attr_v, attr_b, dgeo, amb_attr = _attr_stage(
+            W, enc[r0:r1].repeat_interleave(S, 0), enc_e[r0:r1].repeat_interleave(S, 0), f["geo"], lv,
+            up["dattr"][:, p0:p1], up["dattr_e"][:, p0:p1], tid, tc, tiles, gA1, gA2, gA3)
+        n_amb += int(f["amb1"].any(1).sum())
         n_amb_attr += int(amb_attr.sum())
-        # ---- backward: attribute heads ----
-        dgeo = None
-        for net in range(2):
-            h1, on_a1, amb_a1, h2, on_a2, amb_a2, s, sb = heads[net]
-            da, dae = up["dattr"][net, p0:p1], up["dattr_e"][net, p0:p1]
-            q = s * (1 - s)
-            dl = V((da * q)[:, None],
-                   (q * dae + da.abs() * ((1 - 2 * s).abs() * sb + sb * sb) + _round((da * q).abs(), 4.0))[:, None])
-            w3 = W[f"a3_{net}"][0]
-            if tc:          # dO8 and T3 tiles: scaled by cs from amax(|dl|) max(1, max|w3|)
-                am = _tiles_dense(_row_amax(dl), S) * max(1.0, float(w3.abs().max()))
-                dl = _rescale(dl, am)
-            gA3[net].add(dl, h2, tid)
-            d2 = V(dl.v * w3, dl.e * w3.abs() + _round(dl.mag() * w3.abs(), 1.0))
-            if tc:
-                d2 = _rescale(d2, am)
-            d2 = _mask(d2, on_a2, amb_a2)
-            gA2[net].add(d2, h1, tid)
-            d1 = _back(d2, W[f"a2_{net}"], 64, on_a1, amb_a1)
-            if tc:
-                d1 = _rescale(d1, _tiles_dense(_row_amax(d1), S))
-            gA1[net].add(d1, a_in, tid)
-            g = _back(d1, W[f"a1_{net}"][:, ENC:ENC + GEO], 64)
-            dgeo = g if dgeo is None else V(dgeo.v + g.v, dgeo.e + g.e + _round(dgeo.mag() + g.mag(), 1.0))
-        # ---- backward: sigma MLP ----
-        eo = o.v[:, 0].clamp(-15.0, 15.0).exp()
-        ds, dse = up["dsig"][p0:p1], up["dsig_e"][p0:p1]
-        d0 = V((ds * eo)[:, None], (dse * eo + ds.abs() * eo * torch.expm1(o.e[:, 0]) + _round((ds * eo).abs(), 3.0))[:, None])
-        do = V(torch.cat([d0.v, dgeo.v], 1), torch.cat([d0.e, dgeo.e], 1))
-        if tc:
-            do = _rescale(do, _tiles_dense(_row_amax(do), S))
-            lsc = pow2_log2(_tiles_dense(do.v.abs().amax(1), S))
-        gS2.add(do, h, tid)
-        dh = _back(do, W["s2"], 16, on1, amb1)
-        if tc:              # sc r of the sigma backward's two delta tiles, from the reference's tile maxima
-            lr = pow2_log2(_tiles_dense(dh.v.abs().amax(1), S) * torch.exp2(lsc))
-            live_t = (lsc > 0) & (lr > 0)
-            if bool(live_t.any()):
-                max_log2_scale = max(max_log2_scale, float((lsc + lr)[live_t].max()))
-            dh = _rescale(dh, _tiles_dense(_row_amax(dh), S))
-        gS1.add(dh, xt, tid)
-        dx = _back(dh, W["s1"][:, :K], 64)
+        dx, lsc = _sigma_backward(W, K, f, up["dsig"][p0:p1], up["dsig_e"][p0:p1], dgeo, tid, tc, tiles, gS1, gS2)
+        max_log2_scale = max(max_log2_scale, lsc)
         if on_chunk is not None:
-            on_chunk(p0, p1, {"sigma": (sig, sig_b), "attr": (torch.stack(attr_v), torch.stack(attr_b)),
-                              "geo": (geo.v, geo.e), "dfeat": (dx.v, dx.e)})
+            on_chunk(p0, p1, {"sigma": (f["sig"], f["sig_b"]), "attr": (attr_v, attr_b),
+                              "geo": (f["geo"].v, f["geo"].e), "dfeat": (dx.v, dx.e)})
     T = n_rays * ((S + TILE - 1) // TILE)
     out = {"ambiguous": n_amb, "ambiguous_attr": n_amb_attr, "tiles": T, "max_log2_scale": max_log2_scale}
     v1, b1 = gS1.result()
     v2, b2 = gS2.result()
     out["sigma_net.params"] = (torch.cat([v1.reshape(-1), v2.reshape(-1)]), torch.cat([b1.reshape(-1), b2.reshape(-1)]))
-    for net, name in enumerate(HEADS):
-        parts = [gA1[net].result(), gA2[net].result(), gA3[net].result()]
-        z = torch.zeros(15 * 64, dtype=torch.float64, device=dev)         # W3 rows 1..15: no contribution
-        out[name] = (torch.cat([p[0].reshape(-1) for p in parts] + [z]), torch.cat([p[1].reshape(-1) for p in parts] + [z]))
+    _head_results(gA1, gA2, gA3, out, dev)
+    return out
+
+
+# ---- the point queries: LiDAR4D.density and LiDAR4D.attribute (csrc/l4d_points.cuh) ------------------------------------
+def _point_chunk(chunk: int) -> int:
+    return max(TILE, chunk // TILE * TILE)             # the point kernels' flat tiles start at multiples of 128
+
+
+def density_point_reference(cfg, W: dict, X: torch.Tensor, dsig=None, dgeo=None, on_chunk=None, chunk: int = CHUNK) -> dict:
+    """Float64 sigma MLP of n explicit points, forward and backward (k_density_train's σ / geo from its saved features,
+    k_density_bwd's B1 and B3).  X [n, K] the saved features (exact); dsig [n] and dgeo [n, 15]: the exact upstream
+    gradients, None for a missing one (the kernel then reads a null pointer as 0).  on_chunk(p0, p1, outs) gets sigma [c],
+    geo [c, 15] and dfeat [c, K] (dL/dfeature, which the kernel forms from dh without storing it) as (value, bound).
+    Returns sigma_net.params -> (value, bound) with the point path's rounding depth, "ambiguous" and "tiles"."""
+    dev = X.device
+    n, K = X.shape
+    ip = cfg.sigma_in_pad
+    gS1, gS2 = _Grad((64, ip), dev, POINT_TILE_ROUNDINGS), _Grad((16, 64), dev, POINT_TILE_ROUNDINGS)
+    chunk = _point_chunk(chunk)
+    n_amb = 0
+    for p0 in range(0, n, chunk):
+        p1 = min(n, p0 + chunk)
+        c = p1 - p0
+        tid = torch.arange(c, device=dev) // TILE
+        f = _sigma_forward(W, X[p0:p1], ip)
+        n_amb += int(f["amb1"].any(1).sum())
+        z = torch.zeros(c, dtype=torch.float64, device=dev)
+        ds = z if dsig is None else dsig[p0:p1].double().to(dev)
+        dg = exact(torch.zeros(c, GEO, dtype=torch.float64, device=dev) if dgeo is None else dgeo[p0:p1].to(dev))
+        dx, _ = _sigma_backward(W, K, f, ds, z, dg, tid, False, None, gS1, gS2)
+        if on_chunk is not None:
+            on_chunk(p0, p1, {"sigma": (f["sig"], f["sig_b"]), "geo": (f["geo"].v, f["geo"].e), "dfeat": (dx.v, dx.e)})
+    v1, b1 = gS1.result()
+    v2, b2 = gS2.result()
+    return {"ambiguous": n_amb, "tiles": (n + TILE - 1) // TILE,
+            "sigma_net.params": (torch.cat([v1.reshape(-1), v2.reshape(-1)]), torch.cat([b1.reshape(-1), b2.reshape(-1)]))}
+
+
+def attribute_point_reference(cfg, W: dict, d: torch.Tensor, geo: torch.Tensor, mask, dattr: torch.Tensor, on_chunk=None,
+                              chunk: int = CHUNK) -> dict:
+    """Float64 attribute nets of n explicit points, forward and backward (k_attribute, k_attribute_bwd).  d [n, 3] the
+    directions (encoded per point, direction_encoding), geo [n, 15] exact, mask [n] bool or None (all points), dattr [n, 2]
+    the exact dL/d(raydrop, intensity).  on_chunk(p0, p1, outs) gets attr [2, c] (0 outside the mask) and dgeo [c, 15]
+    (0 outside the mask) as (value, bound).  Returns intensity_net.params and raydrop_net.params -> (value, bound) with
+    the point path's rounding depth, and "ambiguous_attr"."""
+    dev = d.device
+    n = d.shape[0]
+    assert cfg.attr_in_pad == ENC + GEO + 9
+    ap = cfg.attr_in_pad
+    gA1 = [_Grad((64, ap), dev, POINT_TILE_ROUNDINGS) for _ in range(2)]
+    gA2 = [_Grad((64, 64), dev, POINT_TILE_ROUNDINGS) for _ in range(2)]
+    gA3 = [_Grad((1, 64), dev, POINT_TILE_ROUNDINGS) for _ in range(2)]
+    chunk = _point_chunk(chunk)
+    n_amb = 0
+    for p0 in range(0, n, chunk):
+        p1 = min(n, p0 + chunk)
+        c = p1 - p0
+        tid = torch.arange(c, device=dev) // TILE
+        lv = torch.ones(c, dtype=torch.bool, device=dev) if mask is None else mask[p0:p1].to(dev).bool()
+        enc, enc_e = direction_encoding(d[p0:p1])
+        da = dattr[p0:p1].double().t() * lv.double()
+        attr_v, attr_b, dgeo, amb = _attr_stage(W, enc, enc_e, exact(geo[p0:p1]), lv, da, torch.zeros_like(da), tid,
+                                                False, None, gA1, gA2, gA3)
+        n_amb += int(amb.sum())
+        if on_chunk is not None:
+            on_chunk(p0, p1, {"attr": (attr_v, attr_b), "dgeo": (dgeo.v, dgeo.e)})
+    out = {"ambiguous_attr": n_amb, "tiles": (n + TILE - 1) // TILE}
+    _head_results(gA1, gA2, gA3, out, dev)
     return out
 
 
 # ---- the flow MLP ---------------------------------------------------------------------------------------------------------
-def flow_reference(W: dict, fin: torch.Tensor, dflow: torch.Tensor, tc: bool, on_chunk=None, chunk: int = CHUNK) -> dict:
+def flow_reference(W: dict, fin: torch.Tensor, dflow: torch.Tensor, tc: bool, on_chunk=None, chunk: int = CHUNK,
+                   dflow_err: torch.Tensor = None, points: bool = False) -> dict:
     """Float64 flow MLP of P samples, forward and backward.
 
-    fin [16, P] (the forward's flow-MLP input, float32 values), dflow [6, P] (the saved upstream gradient).
+    fin [16, P] (the forward's flow-MLP input, float32 values), dflow [6, P] (the upstream gradient: exact as the kernels
+    saved or received it, or a float64 reference with its bound dflow_err [6, P] - the density backward forms dL/dflow
+    from its own dL/dfeature and never stores it).  points: the weight gradients take the point kernels' rounding depth.
     on_chunk(p0, p1, outs) gets flow [c, 6] and dfin [c, 16] as (value, bound).  Returns flow_net.mlp.{0,2,4}.weight
     -> (value, bound), "ambiguous" and "tiles"."""
     dev = fin.device
     P = fin.shape[1]
-    g0, g1, g2 = _Grad((64, 16), dev), _Grad((64, 64), dev), _Grad((6, 64), dev)
+    per_tile = POINT_TILE_ROUNDINGS if points else 2.0
+    g0, g1, g2 = _Grad((64, 16), dev, per_tile), _Grad((64, 64), dev, per_tile), _Grad((6, 64), dev, per_tile)
     chunk = max(TILE, chunk // TILE * TILE)           # the kernels' flat tiles start at multiples of 128
     n_amb = 0
     for p0 in range(0, P, chunk):
@@ -378,6 +488,8 @@ def flow_reference(W: dict, fin: torch.Tensor, dflow: torch.Tensor, tc: bool, on
         fl = _lin(h2, W["f2"], 64)
         n_amb += int((amb1.any(1) | amb2.any(1)).sum())
         g = exact(dflow[:, p0:p1].t())
+        if dflow_err is not None:
+            g = V(g.v, dflow_err[:, p0:p1].t().double())
         if tc:
             g = _rescale(g, _tiles_flat(_row_amax(g)))
         g2.add(g, h2, tid)

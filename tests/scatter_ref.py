@@ -112,6 +112,13 @@ def sample_x01(rays_o: torch.Tensor, rays_d: torch.Tensor, z: torch.Tensor, boun
     return ((p + b) / (b * 2.0)).reshape(-1, 3)
 
 
+def point_x01(x: torch.Tensor, bound: float) -> torch.Tensor:
+    """l4d_point_x01 of explicit points x [n, 3]: (x + bound) / (2 bound), float32 op by op, no clamp (points outside the
+    box give coordinates outside [0, 1])."""
+    b = torch.tensor(bound, dtype=torch.float32, device=x.device)
+    return (x.float() + b) / (b * 2.0)
+
+
 def axis(c: torch.Tensor, size: int):
     """l4d_axis: float32 coordinate in [0, 1] -> (i0, i1, w0, w1, gmult) of F.grid_sample(align_corners=True, border)."""
     c = c.float()
@@ -135,21 +142,27 @@ def axis(c: torch.Tensor, size: int):
 
 # ---- accumulation -----------------------------------------------------------------------------------------------------
 class _Sink:
-    """Per-entry (sum, sum of magnitudes, count) in float64."""
+    """Per-entry (sum, sum of magnitudes, count) in float64, and with carry=True a fourth column: the error bound carried
+    in from the contributions' inputs."""
 
-    def __init__(self, n: int, device):
-        self.t = torch.zeros(n, 3, dtype=torch.float64, device=device)
+    def __init__(self, n: int, device, carry: bool = False):
+        self.t = torch.zeros(n, 4 if carry else 3, dtype=torch.float64, device=device)
 
-    def add(self, idx, c, a=None):
+    def add(self, idx, c, a=None, e=None):
         c = c.reshape(-1)
         a = c.abs() if a is None else a.reshape(-1)
-        self.t.index_add_(0, idx.reshape(-1), torch.stack([c, a, torch.ones_like(c)], 1))
+        cols = [c, a, torch.ones_like(c)]
+        if self.t.shape[1] > 3:
+            cols.append(torch.zeros_like(c) if e is None else e.reshape(-1))
+        self.t.index_add_(0, idx.reshape(-1), torch.stack(cols, 1))
 
     def scaled(self, f: float):
         """The entries times a constant factor f (exact in float64 up to 2^-53)."""
         t = self.t.clone()
         t[:, 0] *= f
         t[:, 1] *= abs(f)
+        if t.shape[1] > 3:
+            t[:, 3] *= abs(f)
         return t
 
 
@@ -165,16 +178,20 @@ def _texels(Pt, b):
     return Pt[ys, xs], wx * wy, ys, xs
 
 
-def scatter_reference(cfg, params: dict, frame, x01: torch.Tensor, dfeat: torch.Tensor, flow: torch.Tensor,
-                      dfin: torch.Tensor = None, dfin_err: torch.Tensor = None) -> dict:
+def scatter_reference(cfg, params: dict, frame, x01: torch.Tensor, dfeat, flow, dfin: torch.Tensor = None,
+                      dfin_err: torch.Tensor = None, dfeat_err: torch.Tensor = None) -> dict:
     """Float64 reference of the scatter stage.
 
     cfg FieldConfig; params: name -> fp32 master tensor (reference state_dict names); frame: geometry.FrameConstants;
-    x01 [P, 3] float32 (sample_x01); dfeat [P, sigma_in_dim] float32; flow [6, P] float32 (the forward's);
+    x01 [P, 3] float32 (sample_x01 or point_x01); dfeat [P, sigma_in_dim] float32; flow [6, P] float32 (the forward's);
     dfin [16, P] dL/d(flow-MLP input) or None (no flow-grid reference): the kernel's saved float32 values, or a float64
     reference with its error bound dfin_err [16, P] (tests/dense_ref.py, for the fp32 kernels, which never store it).
-    Returns name -> [numel, 3] float64 (ref, A, n) per entry in the tensor's flat order, and "dflow" -> [P, 6, 3]; with
-    dfin_err the flow grid's entries get a fourth column, the bound carried in from dfin_err (check_entries adds it)."""
+    dfeat_err [P, sigma_in_dim]: dfeat is itself a float64 reference with this bound (the point density backward forms
+    dL/dfeature from dh without storing it); every table entry and dL/dflow then carry it in a fourth column.
+    dfeat None: the flow grid alone, from a dfin produced after a first pass (the density backward's order is
+    dL/dfeature -> dL/dflow -> dL/d(flow-MLP input) -> flow grid).
+    Returns name -> [numel, 3] float64 (ref, A, n) per entry in the tensor's flat order, and "dflow" -> [P, 6, 3]; a fourth
+    column holds a carried-in bound where dfin_err (flow grid) or dfeat_err (the others) is given (check_entries adds it)."""
     dev = x01.device
     P = x01.shape[0]
     nS, L = cfg.n_levels_plane, cfg.n_levels_hash
@@ -187,41 +204,28 @@ def scatter_reference(cfg, params: dict, frame, x01: torch.Tensor, dfeat: torch.
         queries.append((1, 0.25, frame.fwd))
     if frame.has_bwd:
         queries.append((2, 0.25, frame.bwd))
+    feats = dfeat is not None
+    carry = dfeat_err is not None
 
     gs, gf = cfg.static_grid(), cfg.flow_grid()
     gd = [cfg.dynamic_grid(p) for p in range(3)]
-    static = _Sink(int(gs.offset[-1]) * 4, dev)
-    comb = [_Sink(int(gd[p].offset[-1]), dev) for p in range(3)]        # sum of w_corner * wc * dL/dfeature
     fcomb = _Sink(int(gf.offset[-1]) * 2, dev) if dfin is not None else None
     ferr = torch.zeros(int(gf.offset[-1]) * 2, dtype=torch.float64, device=dev) if dfin_err is not None else None
     planes, pl64 = {}, {}
-    for s in range(nS):
-        for ci in range(6):
-            name = f"planes_encoder.planes.{s}.{ci}"
-            planes[name] = _Sink(params[name].numel(), dev)
-            pl64[name] = params[name].detach()[0].permute(1, 2, 0).double()         # [H, W, 8]
-    dflow = torch.zeros(P, 6, 3, dtype=torch.float64, device=dev)
+    if feats:
+        static = _Sink(int(gs.offset[-1]) * 4, dev, carry)
+        comb = [_Sink(int(gd[p].offset[-1]), dev, carry) for p in range(3)]    # sum of w_corner * wc * dL/dfeature
+        for s in range(nS):
+            for ci in range(6):
+                name = f"planes_encoder.planes.{s}.{ci}"
+                planes[name] = _Sink(params[name].numel(), dev, carry)
+                pl64[name] = params[name].detach()[0].permute(1, 2, 0).double()         # [H, W, 8]
+        dflow = torch.zeros(P, 6, 4 if carry else 3, dtype=torch.float64, device=dev)
     ar4 = torch.arange(4, device=dev)
 
     for h in range(0, P, CHUNK):
         x = x01[h:h + CHUNK].float()
         C = x.shape[0]
-        d = dfeat[h:h + CHUNK].double()
-        fl = flow[:, h:h + CHUNK].t().float()
-        warped = {0: x, 1: x + fl[:, 0:3], 2: x + fl[:, 3:6]}                    # float32 adds, as the kernels
-
-        # static hash: entry (offset[l] + idx) * 4 + f gets w_corner * dL/dfeature[row_hash_s + 4 l + f]
-        for l in range(L):
-            idx, w = O.hash_indices(x, gs, l)
-            ent = ((idx + int(gs.offset[l])) * 4)[:, :, None] + ar4
-            static.add(ent, w.double()[:, :, None] * d[:, None, row_hash_s + 4 * l:row_hash_s + 4 * l + 4])
-
-        # dynamic hash, current query: one sum per entry; the time basis and slice weights are constants of the launch
-        for p, (a, b) in enumerate(DYN_PAIRS):
-            x2 = x[:, [a, b]]
-            for l in range(L):
-                idx, w = O.hash_indices(x2, gd[p], l)
-                comb[p].add(idx + int(gd[p].offset[l]), w.double() * (wc * d[:, row_hash_d + p * L + l:row_hash_d + p * L + l + 1]))
 
         # flow grid: feature (l, 2i + c) of a corner gets basis[i] * w_corner * dFin[2l + c]; the basis is applied below
         if fcomb is not None:
@@ -233,11 +237,34 @@ def scatter_reference(cfg, params: dict, frame, x01: torch.Tensor, dfeat: torch.
                 if ferr is not None:
                     dfe = dfin_err[2 * l:2 * l + 2, h:h + CHUNK].t().double()
                     ferr.index_add_(0, ent.reshape(-1), (w.double()[:, :, None] * dfe[:, None, :]).reshape(-1))
+        if not feats:
+            continue
+
+        d = dfeat[h:h + CHUNK].double()
+        de = dfeat_err[h:h + CHUNK].double() if carry else torch.zeros_like(d)
+        fl = flow[:, h:h + CHUNK].t().float()
+        warped = {0: x, 1: x + fl[:, 0:3], 2: x + fl[:, 3:6]}                    # float32 adds, as the kernels
+
+        # static hash: entry (offset[l] + idx) * 4 + f gets w_corner * dL/dfeature[row_hash_s + 4 l + f]
+        for l in range(L):
+            idx, w = O.hash_indices(x, gs, l)
+            ent = ((idx + int(gs.offset[l])) * 4)[:, :, None] + ar4
+            sl = slice(row_hash_s + 4 * l, row_hash_s + 4 * l + 4)
+            wd = w.double()[:, :, None]
+            static.add(ent, wd * d[:, None, sl], e=wd * de[:, None, sl])
+
+        # dynamic hash, current query: one sum per entry; the time basis and slice weights are constants of the launch
+        for p, (a, b) in enumerate(DYN_PAIRS):
+            x2 = x[:, [a, b]]
+            for l in range(L):
+                idx, w = O.hash_indices(x2, gd[p], l)
+                r = row_hash_d + p * L + l
+                comb[p].add(idx + int(gd[p].offset[l]), w.double() * (wc * d[:, r:r + 1]), e=w.double() * (wc * de[:, r:r + 1]))
 
         for s in range(nS):
             R = cfg.min_resolution * cfg.plane_scales[s]
             # static planes: product rule over (x,y) (x,z) (y,z)
-            ds = d[:, s * 8:s * 8 + 8]
+            ds, dse = d[:, s * 8:s * 8 + 8], de[:, s * 8:s * 8 + 8]
             samp = {}
             for ci in STATIC_PLANES:
                 ca, cb = STATIC_COORDS[ci]
@@ -248,11 +275,14 @@ def scatter_reference(cfg, params: dict, frame, x01: torch.Tensor, dfeat: torch.
                 o1, o2 = OTHER_STATIC[ci]
                 g = ds * samp[o1][0] * samp[o2][0]
                 ga = ds.abs() * samp[o1][1] * samp[o2][1]
+                ge = dse * samp[o1][1] * samp[o2][1]
                 _, _, wgt, ys, xs, W = samp[ci]
                 ent = torch.arange(8, device=dev)[None, None, :] * (R * R) + (ys * W + xs)[:, :, None]
-                planes[f"planes_encoder.planes.{s}.{ci}"].add(ent, wgt[:, :, None] * g[:, None, :], wgt[:, :, None] * ga[:, None, :])
+                planes[f"planes_encoder.planes.{s}.{ci}"].add(ent, wgt[:, :, None] * g[:, None, :], wgt[:, :, None] * ga[:, None, :],
+                                                              wgt[:, :, None] * ge[:, None, :])
             # time planes (x,t) (y,t) (z,t) at every live query; the warped queries also give dL/dflow
             dt = d[:, row_plane_d + s * 8:row_plane_d + s * 8 + 8]
+            dte = de[:, row_plane_d + s * 8:row_plane_d + s * 8 + 8]
             for qi, wq, q in queries:
                 pos = warped[qi]
                 tau = torch.full((1,), float(q.tau), dtype=torch.float32, device=dev)
@@ -277,28 +307,35 @@ def scatter_reference(cfg, params: dict, frame, x01: torch.Tensor, dfeat: torch.
                     o1, o2 = [u for u in range(3) if u != t]
                     g = (wq * dt) * samp[o1][0] * samp[o2][0]
                     ga = (wq * dt).abs() * samp[o1][1] * samp[o2][1]
+                    ge = (wq * dte) * samp[o1][1] * samp[o2][1]
                     _, _, wgt, ys, xs, dx, dxa = samp[t]
                     ent = torch.arange(8, device=dev)[None, None, :] * (T * R) + (ys * R + xs)[:, :, None]
-                    planes[f"planes_encoder.planes.{s}.{ci}"].add(ent, wgt[:, :, None] * g[:, None, :], wgt[:, :, None] * ga[:, None, :])
+                    planes[f"planes_encoder.planes.{s}.{ci}"].add(ent, wgt[:, :, None] * g[:, None, :], wgt[:, :, None] * ga[:, None, :],
+                                                                  wgt[:, :, None] * ge[:, None, :])
                     if qi:
                         k = 3 * (qi - 1) + t
                         dflow[h:h + C, k, 0] += (g * dx).sum(1)
                         dflow[h:h + C, k, 1] += (ga * dxa).sum(1)
                         dflow[h:h + C, k, 2] += 16.0          # 8 channels x 2 texel columns
+                        if carry:
+                            dflow[h:h + C, k, 3] += (ge * dxa).sum(1)
 
-    out = {"hash_encoder.hash_static.params": static.t}
-    out.update({k: v.t for k, v in planes.items()})
-    cur = frame.cur
-    for p in range(3):
-        ne = int(gd[p].offset[-1])
-        for sl in range(T):
-            wsl = (1.0 if sl == cur.slice_lo else 0.0) if cur.single else \
-                (float(cur.w_lo) if sl == cur.slice_lo else (float(cur.w_hi) if sl == cur.slice_hi else 0.0))
-            t = torch.zeros(ne, 4, 3, dtype=torch.float64, device=dev)
-            if wsl != 0.0:
-                for k in range(4):
-                    t[:, k] = comb[p].scaled(wsl * float(cur.basis[k]))
-            out[f"hash_encoder.hash_dynamic.{p}.hash_t.{sl}.params"] = t.view(-1, 3)
+    out = {}
+    if feats:
+        out["hash_encoder.hash_static.params"] = static.t
+        out.update({k: v.t for k, v in planes.items()})
+        cur = frame.cur
+        for p in range(3):
+            ne = int(gd[p].offset[-1])
+            for sl in range(T):
+                wsl = (1.0 if sl == cur.slice_lo else 0.0) if cur.single else \
+                    (float(cur.w_lo) if sl == cur.slice_lo else (float(cur.w_hi) if sl == cur.slice_hi else 0.0))
+                t = torch.zeros(ne, 4, comb[p].t.shape[1], dtype=torch.float64, device=dev)
+                if wsl != 0.0:
+                    for k in range(4):
+                        t[:, k] = comb[p].scaled(wsl * float(cur.basis[k]))
+                out[f"hash_encoder.hash_dynamic.{p}.hash_t.{sl}.params"] = t.view(ne * 4, -1)
+        out["dflow"] = dflow
     if fcomb is not None:
         ne = int(gf.offset[-1])
         nc = 3 if ferr is None else 4
@@ -312,7 +349,6 @@ def scatter_reference(cfg, params: dict, frame, x01: torch.Tensor, dfeat: torch.
             if ferr is not None:
                 t[:, i, :, 3] = ferr.view(ne, 2) * abs(bi)
         out["flow_net.grid_enc.params"] = t.view(-1, nc)
-    out["dflow"] = dflow
     return out
 
 

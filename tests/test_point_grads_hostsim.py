@@ -221,3 +221,139 @@ def test_point_entry_points_exported_and_checked():
     # n == 0 is a no-op once the arguments are valid
     assert lib.l4d_attribute_backward(C.byref(cc), fake, fake, fake, None, 0, fake, None, C.byref(heads), fake, wb, st) == 0
     assert lib.l4d_density_backward(C.byref(cc), fake, C.byref(fr), fake, 0, fake, 0, fake, None, C.byref(full), fake, wb, st) == 0
+
+
+# ---- the float64 point references (tests/dense_ref.py, tests/points_check.py) ------------------------------------------
+def _hs_flow(hs, x, t, g_flow):
+    """host-sim l4d_flow_forward (with its saved flow-MLP input) + l4d_flow_backward"""
+    fr = hs.frame(t)
+    x = x.float().contiguous()
+    n = x.shape[0]
+    flow, fin = torch.zeros(n, 6), torch.zeros(16, n)
+    assert hs.L.hs_flow_forward(C.byref(hs.ccfg), hs.staged.data_ptr(), C.byref(fr), x.data_ptr(), n, flow.data_ptr(),
+                                fin.data_ptr()) == 0
+    grads, tab, work = _grad_tables(hs)
+    g = g_flow.float().contiguous()
+    assert hs.L.hs_flow_backward(C.byref(hs.ccfg), hs.staged.data_ptr(), C.byref(fr), x.data_ptr(), n, fin.data_ptr(),
+                                 g.data_ptr(), C.byref(tab), work.data_ptr()) == 0
+    assert hs.L.hs_unstage_grads(C.byref(hs.ccfg), work.data_ptr(), C.byref(tab)) == 0
+    return flow, fin, grads
+
+
+def _hs_density_saved(hs, x, t, g_sigma, g_geo):
+    """hs_density_grads that also returns the saved flow-MLP input and features"""
+    import points_check as PC
+    fr = hs.frame(t)
+    x = x.float().contiguous()
+    n = x.shape[0]
+    out = dict(sigma=torch.zeros(n), geo_feat=torch.zeros(n, 15), features=torch.zeros(n, hs.cfg.sigma_in_dim),
+               flow=torch.zeros(n, 6))
+    saved = torch.zeros(PH.lib().hs_density_saved_bytes(C.byref(hs.ccfg), n), dtype=torch.uint8)
+    assert PH.lib().hs_density_forward_ex(C.byref(hs.ccfg), hs.staged.data_ptr(), C.byref(fr), x.data_ptr(), n,
+                                          out["sigma"].data_ptr(), out["geo_feat"].data_ptr(), out["features"].data_ptr(),
+                                          out["flow"].data_ptr(), saved.data_ptr()) == 0
+    grads, tab, work = _grad_tables(hs)
+    gs = None if g_sigma is None else g_sigma.float().contiguous()
+    gg = None if g_geo is None else g_geo.float().contiguous()
+    assert PH.lib().hs_density_backward(C.byref(hs.ccfg), hs.staged.data_ptr(), C.byref(fr), x.data_ptr(), n,
+                                        saved.data_ptr(), gs.data_ptr() if gs is not None else None,
+                                        gg.data_ptr() if gg is not None else None, C.byref(tab), work.data_ptr()) == 0
+    assert hs.L.hs_unstage_grads(C.byref(hs.ccfg), work.data_ptr(), C.byref(tab)) == 0
+    fin, feat = PC.density_saved_views(hs.cfg, saved, n)
+    return out, fin.clone(), feat.clone(), grads
+
+
+@pytest.mark.parametrize("t", TIMES)
+def test_point_references_equal_autograd(t):
+    """density_point_reference, flow_reference and attribute_point_reference against torch.autograd.grad through the
+    float64 oracle on the same inputs: features, flow-MLP inputs, directions and geo.  The density / flow values agree
+    to float64 rounding (the references' inputs are the oracle's own); the attribute nets agree within the reference's
+    bound (the oracle rounds the direction encoding's sine to float32, the reference keeps it in float64)."""
+    import dense_ref as DR
+    cfg = small_config()
+    orc = O.build_seeded(cfg, 21, flow_last_std=0.05)
+    params32 = {k: v.detach().clone().float() for k, v in orc.ref_state_dict().items()}
+    orc.to_float64()
+    fr = make_frame(t, cfg.num_frames, cfg.time_resolution)
+    g = torch.Generator().manual_seed(3)
+    n = 700
+    x = torch.rand(n, 3, generator=g) * 2 - 1
+    out = orc.density(x, fr, return_features=True)
+    gs, gg, gf = (torch.randn(n, generator=g).double(), torch.randn(n, 15, generator=g).double(),
+                  torch.randn(n, 6, generator=g).double())
+    feats, fin = out["features"], out["flow_in"]
+    names = ["sigma_net.params", "flow_net.mlp.0.weight", "flow_net.mlp.2.weight", "flow_net.mlp.4.weight"]
+    loss = (out["sigma"] * gs).sum() + (out["geo_feat"] * gg).sum() + (out["flow"] * gf).sum()
+    want = torch.autograd.grad(loss, [orc.p(k) for k in names] + [feats, fin])
+    W = DR.working_weights(cfg, params32, False)
+    kept = {}
+    dref = DR.density_point_reference(cfg, W, feats.detach(), gs, gg, lambda p0, p1, o: kept.update(o))
+    fref = DR.flow_reference(W, fin.detach().t(), gf.t(), False, lambda p0, p1, o: kept.update(o), points=True)
+    # loss reaches the flow MLP both through flow (gf) and, via the features, through the warped queries; the flow
+    # reference takes the first part only, so compare it with autograd of (flow * gf) alone
+    want_flow = torch.autograd.grad((orc.density(x, fr, return_features=True)["flow"] * gf).sum(),
+                                    [orc.p(k) for k in names[1:]])
+
+    def close(got, ref, bound, what):
+        err = (got.double().reshape(-1) - ref.double().reshape(-1)).abs()
+        tol = 1e-9 * bound.reshape(-1) + 1e-12 * float(ref.detach().abs().max())
+        assert bool((err <= tol).all()), (what, float(err.max()), float(bound.max()))
+    close(kept["sigma"][0], out["sigma"], kept["sigma"][1], "sigma")
+    close(kept["geo"][0], out["geo_feat"], kept["geo"][1], "geo")
+    close(kept["dfeat"][0], want[-2], kept["dfeat"][1], "dfeat")
+    close(dref["sigma_net.params"][0], want[0], dref["sigma_net.params"][1], "sigma_net.params")
+    close(kept["flow"][0], out["flow"], kept["flow"][1], "flow")
+    for k, w in zip(names[1:], want_flow):
+        close(fref[k][0], w, fref[k][1], k)
+    assert float(dref["sigma_net.params"][0].abs().max()) > 0 and float(fref[names[1]][0].abs().max()) > 0
+    # attribute nets on a partial mask
+    d = torch.nn.functional.normalize(torch.randn(n, 3, generator=g), dim=-1)
+    d[:6] = torch.tensor([[1.0, 0, 0], [-1.0, 0, 0], [0, 1.0, 0], [0, -1.0, 0], [0, 0, 1.0], [0, 0, -1.0]])
+    geo = torch.randn(n, 15, generator=g).double()
+    mask = torch.rand(n, generator=g) > 0.3
+    go = torch.randn(n, 2, generator=g).double()
+    geo_t = geo.clone().requires_grad_(True)
+    a = orc.attribute(d, geo_t, mask)
+    heads = [orc.p(k) for k in DR.HEADS]
+    wa = torch.autograd.grad((a * go).sum(), heads + [geo_t])
+    aref = DR.attribute_point_reference(cfg, W, d, geo, mask, go, lambda p0, p1, o: kept.update(o))
+    for got, ref, b, what in [(kept["attr"][0].t(), a, kept["attr"][1].t(), "attr"),
+                              (kept["dgeo"][0], wa[-1], kept["dgeo"][1], "dgeo")] + \
+            [(aref[k][0], w, aref[k][1], k) for k, w in zip(DR.HEADS, wa)]:
+        err = (got.reshape(-1) - ref.detach().double().reshape(-1)).abs()
+        assert bool((err <= b.reshape(-1) + 1e-12 * float(ref.detach().abs().max())).all()), \
+            (what, float((err - b.reshape(-1)).max()))
+    assert float(kept["attr"][0][:, ~mask].abs().max()) == 0 and float(kept["dgeo"][0][~mask].abs().max()) == 0
+
+
+@pytest.mark.parametrize("fp16", [False, True])
+@pytest.mark.parametrize("t", TIMES)
+def test_host_build_within_point_bounds(t, fp16):
+    """The host build of the point kernels (float32, contraction off) stays inside every bound of tests/points_check.py:
+    flow, density and attribute, forward and backward, on 300 points in and outside the box (|x| up to 1.5 bound)."""
+    import points_check as PC
+    cfg = small_config(bound=0.75)
+    orc = O.build_seeded(cfg, 21, flow_last_std=0.02)
+    if fp16:
+        orc.mlp_dtype = "fp16"
+    hs = H.HostSim(orc, mlp_fp16=fp16)
+    params = hs.params
+    g = torch.Generator().manual_seed(6)
+    n = 300
+    x = (torch.rand(n, 3, generator=g) * 3 - 1.5) * cfg.bound
+    gf = torch.randn(n, 6, generator=g)
+    flow, fin, grads = _hs_flow(hs, x, t, gf)
+    st = PC.hold_flow(cfg, params, fp16, t, x, flow, fin, gf, grads, what=f"host flow t={t}")
+    gs, gg = torch.randn(n, generator=g), torch.randn(n, 15, generator=g)
+    out, fin, feat, grads = _hs_density_saved(hs, x, t, gs, gg)
+    sd = PC.hold_density(cfg, params, fp16, t, x, out, fin, feat, gs, gg, grads, what=f"host density t={t}")
+    d = torch.nn.functional.normalize(torch.randn(n, 3, generator=g), dim=-1)
+    geo = out["geo_feat"]
+    mask = torch.rand(n, generator=g) > 0.4
+    go = torch.randn(n, 2, generator=g)
+    g_geo, grads = hs_attribute_grads(hs, d, geo, mask, go)
+    # the host build has no attribute forward entry point: its forward is held on the GPU only
+    sa = PC.hold_attribute(cfg, params, fp16, d, geo, mask, None, go, g_geo, grads, what="host attribute")
+    assert st["ambiguous"] + sd["ambiguous"] <= PC.MAX_AMBIGUOUS * 2 * n, (st["ambiguous"], sd["ambiguous"])
+    print(f"[points-host] t={t} fp16={fp16}: flow {st['holder'].line()}; density {sd['holder'].line()}; "
+          f"attribute {sa['holder'].line()}")
