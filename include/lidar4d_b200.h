@@ -282,6 +282,55 @@ int    l4d_attribute_backward(const L4DConfig* cfg, const void* staged, const fl
                               float* g_geo_or_null, const L4DMasterGrads* grads,
                               void* grad_work, size_t grad_work_bytes, void* stream);
 
+/* --- LiDAR4D's submodules called on their own (hash_field.py, planes_field.py, flow_field.py, the tcnn encodings and
+ *     networks): inputs row-major fp32 in [0,1] (no bound normalisation; points outside are encoded as tcnn and
+ *     grid_sample encode them), outputs row-major fp32, the staged working set of the render path (fp16 tables, MLP
+ *     working copies of the precision mode).  Both families: null or not 4-byte aligned pointers, an unknown module / net
+ *     or n > 2^31: L4D_EINVAL; n == 0 is a no-op without a launch; one launch on `stream`.  The backwards ACCUMULATE
+ *     (hash tables straight into `grads`, planes and MLP weights into `grad_work`; the caller runs l4d_unstage_grads).
+ * l4d_encoder_forward(module, query, slice, x[n, in], out[n, out]); (in -> out) per module, L = hash levels, S = plane
+ *     scales:
+ *       L4D_MOD_HASH_STATIC      x[n,3]  -> [n, 4L]    hash_encoder.hash_static
+ *       L4D_MOD_HASH_T0 + p      x[n,2]  -> [n, L]     hash_encoder.hash_dynamic[p] at `query` (p: 0 xy, 1 xz, 2 yz)
+ *       L4D_MOD_HASH_DYNAMIC     x[n,3]  -> [n, 3L]    hash_encoder.forward_dynamic at `query`
+ *       L4D_MOD_HASH_SLICE0 + p  x[n,2]  -> [n, 4L]    hash_encoder.hash_dynamic[p].hash_t[slice]
+ *       L4D_MOD_PLANES_STATIC    xt[n,4] -> [n, 8S]    planes_encoder.forward_static
+ *       L4D_MOD_PLANES_DYNAMIC   xt[n,4] -> [n, 8S]    planes_encoder.forward_dynamic (time = column 3 of each row)
+ *       L4D_MOD_FLOW_GRID        x[n,3]  -> [n, 64]    flow_net.grid_enc
+ *       L4D_MOD_FLOW             xt[n,4] -> [n, 6]     flow_net; the time of EVERY row is xt[0,3], read on the device
+ *       L4D_MOD_FREQ             v[n,3]  -> [n, 72]    view_encoder (degree 12)
+ *     `query` is required by the two HASH_T / HASH_DYNAMIC kinds (ignored otherwise), `slice` < time_resolution by
+ *     HASH_SLICE.
+ * l4d_encoder_backward: upstream g_out[n, out] with the inputs of the forward.  Parameter gradients of the module; the
+ *     planes also give dL/dxt into g_x[n,4] when it is not NULL (g_x must be NULL for every other module).  The FREQ
+ *     encoding has no parameters (L4D_EINVAL).  The module's buffers of `grads` must be set.
+ * l4d_mlp_forward(net, in[n, n_in], out[n, n_out]): net L4D_NET_SIGMA (n_in = sigma_in_dim, n_out = 16),
+ *     L4D_NET_RAYDROP / L4D_NET_INTENSITY (n_in = attr_in_dim, n_out = 1: before LiDAR4D.attribute's sigmoid).  Inputs
+ *     are padded with ones to the network width.
+ * l4d_mlp_backward: upstream g_out[n, n_out]; weight gradients of the net, dL/din into g_in[n, n_in] when not NULL. */
+#define L4D_MOD_HASH_STATIC    0u
+#define L4D_MOD_HASH_T0        1u   /* 1..3 */
+#define L4D_MOD_HASH_DYNAMIC   4u
+#define L4D_MOD_HASH_SLICE0    5u   /* 5..7 */
+#define L4D_MOD_PLANES_STATIC  8u
+#define L4D_MOD_PLANES_DYNAMIC 9u
+#define L4D_MOD_FLOW_GRID      10u
+#define L4D_MOD_FLOW           11u
+#define L4D_MOD_FREQ           12u
+#define L4D_NET_SIGMA          0u
+#define L4D_NET_RAYDROP        1u
+#define L4D_NET_INTENSITY      2u
+int    l4d_encoder_forward(const L4DConfig* cfg, const void* staged, uint32_t module, const L4DTimeQuery* query_or_null,
+                           uint32_t slice, const float* x, uint32_t n, float* out, void* stream);
+int    l4d_encoder_backward(const L4DConfig* cfg, const void* staged, uint32_t module, const L4DTimeQuery* query_or_null,
+                            uint32_t slice, const float* x, uint32_t n, const float* g_out, float* g_x_or_null,
+                            const L4DMasterGrads* grads, void* grad_work, size_t grad_work_bytes, void* stream);
+int    l4d_mlp_forward(const L4DConfig* cfg, const void* staged, uint32_t net, const float* in, uint32_t n, float* out,
+                       void* stream);
+int    l4d_mlp_backward(const L4DConfig* cfg, const void* staged, uint32_t net, const float* in, uint32_t n,
+                        const float* g_out, float* g_in_or_null, const L4DMasterGrads* grads, void* grad_work,
+                        size_t grad_work_bytes, void* stream);
+
 /* --- SURVEY 8(f) "next" row 1: the chamfer / nearest-neighbour op of utils/chamfer3D --------------------------
  * Replaces chamfer_cuda.cpp:17-32 `forward(xyz1,xyz2,dist1,dist2,idx1,idx2)` / `backward(...)` (kernels
  * chamfer3D.cu:11-133,154-174).  xyz1[b,n,3], xyz2[b,m,3] fp32 contiguous; dist1[b,n] = squared distance to the

@@ -113,6 +113,16 @@ def make_config(cfg: FieldConfig, mlp_fp16: bool = False) -> L4DConfig:
     return c
 
 
+# module ids of l4d_encoder_forward / l4d_mlp_forward (include/lidar4d_b200.h)
+MOD_HASH_STATIC, MOD_HASH_T0, MOD_HASH_DYNAMIC, MOD_HASH_SLICE0 = 0, 1, 4, 5
+MOD_PLANES_STATIC, MOD_PLANES_DYNAMIC, MOD_FLOW_GRID, MOD_FLOW, MOD_FREQ = 8, 9, 10, 11, 12
+NET_SIGMA, NET_RAYDROP, NET_INTENSITY = 0, 1, 2
+
+
+def make_time_query(q: Optional[TimeQuery]) -> L4DTimeQuery:
+    return _tq(q)
+
+
 def _tq(q: Optional[TimeQuery]) -> L4DTimeQuery:
     s = L4DTimeQuery()
     if q is None:
@@ -148,6 +158,7 @@ EXPORTS = [
     "l4d_flow_forward", "l4d_flow_backward", "l4d_hash_indices", "l4d_density_forward", "l4d_attribute_forward", "l4d_chamfer_work_bytes", "l4d_chamfer_forward", "l4d_chamfer_backward", "l4d_tc_selftest", "l4d_tc_selftest2", "l4d_profile_start", "l4d_profile_stop",
     "l4d_stage_params_ex", "l4d_adam_step", "l4d_launch_count", "l4d_render_backward_ex", "l4d_lidar_rays", "l4d_lidar_loss",
     "l4d_density_saved_bytes", "l4d_density_forward_ex", "l4d_density_backward", "l4d_attribute_backward",
+    "l4d_encoder_forward", "l4d_encoder_backward", "l4d_mlp_forward", "l4d_mlp_backward",
     "l4d_pano_project_work_bytes", "l4d_pano_project", "l4d_pano_unproject_work_bytes", "l4d_pano_unproject",
     "l4d_point_metrics",
     "l4d_range_filter_work_bytes", "l4d_range_filter", "l4d_knn_mean_dist", "l4d_outlier_select_work_bytes",
@@ -254,6 +265,13 @@ def declare(lib, prefix: str = "l4d_", host_sim: bool = False):
         lib.l4d_flow_ground.argtypes = [V, U32, V, V]
         lib.l4d_flow_ground_backward.argtypes = [V, U32, V, V, V]
         lib.l4d_flow_loss_finish.argtypes = [V, U32, U32, V, V]
+        lib.l4d_encoder_forward.argtypes = [P(L4DConfig), V, U32, P(L4DTimeQuery), U32, V, U32, V, V]
+        lib.l4d_encoder_backward.argtypes = [P(L4DConfig), V, U32, P(L4DTimeQuery), U32, V, U32, V, V,
+                                             P(L4DMasterGrads), V, SZ, V]
+        lib.l4d_mlp_forward.argtypes = [P(L4DConfig), V, U32, V, U32, V, V]
+        lib.l4d_mlp_backward.argtypes = [P(L4DConfig), V, U32, V, U32, V, V, P(L4DMasterGrads), V, SZ, V]
+        for n in ("encoder_forward", "encoder_backward", "mlp_forward", "mlp_backward"):
+            getattr(lib, f"l4d_{n}").restype = C.c_int
         for n in ("nn_grid_build", "nn_grid_query", "flow_warp_query", "flow_term_backward", "flow_ground",
                   "flow_ground_backward", "flow_loss_finish"):
             getattr(lib, f"l4d_{n}").restype = C.c_int

@@ -589,13 +589,14 @@ L4D_HD float l4d_x01(float o, float d, float z, float bound) {
   return L4D_DIV(L4D_ADD(p, bound), L4D_MUL(2.0f, bound));
 }
 
-// Frequency encoding of the view direction (per ray): enc[dim*24 + 2k + {0 sin,1 cos}]
-L4D_HD float l4d_freq(float d, int k, int phase) {
-  float v = L4D_DIV(L4D_ADD(d, 1.0f), 2.0f);
+// Frequency encoding (tcnn Frequency) of a coordinate v already in [0,1]: sin(2^k pi v + phase)
+L4D_HD float l4d_freq01(float v, int k, int phase) {
   float xs = L4D_MUL(v, (float)(1u << k));
   float arg = L4D_ADD(L4D_MUL(xs, L4D_PI_F), phase ? L4D_HALF_PI_F : 0.0f);
   return sinf(arg);
 }
+// Frequency encoding of the view direction (per ray): enc[dim*24 + 2k + {0 sin,1 cos}] of (d + 1) / 2
+L4D_HD float l4d_freq(float d, int k, int phase) { return l4d_freq01(L4D_DIV(L4D_ADD(d, 1.0f), 2.0f), k, phase); }
 
 // ---------------------------------------------------------------------------
 // flow field forward (flow_field.py:113-130): grid -> Lagrange -> 16 -> 64 -> 64 -> 6

@@ -1047,6 +1047,7 @@ __global__ void __launch_bounds__(NT) k_attribute(const __grid_constant__ Attrib
 }
 
 #include "l4d_points.cuh"
+#include "l4d_modules.cuh"
 
 // =============================================================================
 // C-ABI launchers
@@ -1661,6 +1662,175 @@ extern "C" int l4d_attribute_backward(const L4DConfig* cfg, const void* staged, 
   rc = grid_for(k_attribute_bwd<L4D_NT>, L4D_NT, smem, (n + L4D_NT - 1) / L4D_NT, grid);
   if (rc != L4D_OK) return rc;
   ++g_launches; k_attribute_bwd<L4D_NT><<<grid, L4D_NT, smem, (cudaStream_t)stream>>>(A);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+// ---- LiDAR4D's submodules on their own (l4d_modules.cuh) -----------------------------------------------------------
+static bool misaligned4(const void* p) { return p && (reinterpret_cast<uintptr_t>(p) & 3u); }
+
+// input / output widths of an encoder module; false for an unknown id
+static bool module_dims(const L4DConfig* cfg, uint32_t module, uint32_t& in, uint32_t& out) {
+  const uint32_t L = cfg->hash_static.n_levels;
+  switch (module) {
+    case L4D_MOD_HASH_STATIC: in = 3; out = 4 * L; return true;
+    case L4D_MOD_HASH_T0: case L4D_MOD_HASH_T0 + 1: case L4D_MOD_HASH_T0 + 2: in = 2; out = L; return true;
+    case L4D_MOD_HASH_DYNAMIC: in = 3; out = 3 * L; return true;
+    case L4D_MOD_HASH_SLICE0: case L4D_MOD_HASH_SLICE0 + 1: case L4D_MOD_HASH_SLICE0 + 2: in = 2; out = 4 * L; return true;
+    case L4D_MOD_PLANES_STATIC: case L4D_MOD_PLANES_DYNAMIC: in = 4; out = 8 * cfg->n_plane_scales; return true;
+    case L4D_MOD_FLOW_GRID: in = 3; out = 8 * cfg->flow.n_levels; return true;
+    case L4D_MOD_FLOW: in = 4; out = 6; return true;
+    case L4D_MOD_FREQ: in = 3; out = L4D_ENC; return true;
+  }
+  return false;
+}
+
+static int module_check(const L4DConfig* cfg, const void* staged, uint32_t module, const L4DTimeQuery* q, uint32_t slice,
+                        const float* x, uint32_t n, ModuleArgs& A) {
+  int rc = check_config(cfg);
+  if (rc != L4D_OK) return rc;
+  if (!staged || !x) return l4d_fail(L4D_EINVAL, "null pointer");
+  if (misaligned4(x)) return l4d_fail(L4D_EINVAL, "misaligned pointer");
+  if (n > (1u << 31)) return l4d_fail(L4D_EINVAL, "n > 2^31");
+  memset(&A, 0, sizeof(A));
+  if (!module_dims(cfg, module, A.in_dim, A.out_dim)) return l4d_fail(L4D_EINVAL, "unknown module id");
+  const bool timed = (module >= L4D_MOD_HASH_T0 && module <= L4D_MOD_HASH_T0 + 2) || module == L4D_MOD_HASH_DYNAMIC;
+  if (timed) {
+    if (!q) return l4d_fail(L4D_EINVAL, "null time query");
+    if (q->slice_lo >= cfg->time_resolution || q->slice_hi >= cfg->time_resolution)
+      return l4d_fail(L4D_EINVAL, "time query slice out of range");
+    A.q = *q;
+  }
+  if (module >= L4D_MOD_HASH_SLICE0 && module <= L4D_MOD_HASH_SLICE0 + 2 && slice >= cfg->time_resolution)
+    return l4d_fail(L4D_EINVAL, "slice out of range");
+  build_model(cfg, staged, A.M);
+  A.module = module; A.slice = slice; A.x = x; A.n = n;
+  return L4D_OK;
+}
+
+extern "C" int l4d_encoder_forward(const L4DConfig* cfg, const void* staged, uint32_t module, const L4DTimeQuery* q,
+                                   uint32_t slice, const float* x, uint32_t n, float* out, void* stream) {
+  ModuleArgs A;
+  int rc = module_check(cfg, staged, module, q, slice, x, n, A);
+  if (rc != L4D_OK) return rc;
+  if (!out) return l4d_fail(L4D_EINVAL, "null pointer");
+  if (misaligned4(out)) return l4d_fail(L4D_EINVAL, "misaligned pointer");
+  if (n == 0) return L4D_OK;
+  A.out = out;
+  const size_t smem = 64 * L4D_NT * sizeof(float);
+  int grid;
+  rc = grid_for(k_module_fwd<L4D_NT>, L4D_NT, smem, (n + L4D_NT - 1) / L4D_NT, grid);
+  if (rc != L4D_OK) return rc;
+  ++g_launches; k_module_fwd<L4D_NT><<<grid, L4D_NT, smem, (cudaStream_t)stream>>>(A);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+extern "C" int l4d_encoder_backward(const L4DConfig* cfg, const void* staged, uint32_t module, const L4DTimeQuery* q,
+                                    uint32_t slice, const float* x, uint32_t n, const float* g_out, float* g_x,
+                                    const L4DMasterGrads* grads, void* grad_work, size_t grad_work_bytes, void* stream) {
+  ModuleArgs A;
+  int rc = module_check(cfg, staged, module, q, slice, x, n, A);
+  if (rc != L4D_OK) return rc;
+  if (module == L4D_MOD_FREQ) return l4d_fail(L4D_EINVAL, "the frequency encoding has no parameters");
+  if (!g_out || !grads || !grad_work) return l4d_fail(L4D_EINVAL, "null pointer");
+  if (misaligned4(g_out) || misaligned4(g_x) || misaligned4(grad_work)) return l4d_fail(L4D_EINVAL, "misaligned pointer");
+  const bool planes = module == L4D_MOD_PLANES_STATIC || module == L4D_MOD_PLANES_DYNAMIC;
+  if (g_x && !planes) return l4d_fail(L4D_EINVAL, "only the planes give an input gradient");
+  if (grad_work_bytes < grad_work_layout(cfg).total) return l4d_fail(L4D_ESIZE, "grad_work buffer too small");
+  // the module's gradient buffers
+  switch (module) {
+    case L4D_MOD_HASH_STATIC:
+      if (!grads->hash_static) return l4d_fail(L4D_EINVAL, "null hash_static gradient buffer");
+      break;
+    case L4D_MOD_FLOW_GRID:
+    case L4D_MOD_FLOW:
+      if (!grads->flow_grid) return l4d_fail(L4D_EINVAL, "null flow_grid gradient buffer");
+      if (module == L4D_MOD_FLOW)
+        for (int k = 0; k < 3; ++k)
+          if (!grads->flow_mlp[k]) return l4d_fail(L4D_EINVAL, "null flow_mlp gradient buffer");
+      break;
+    case L4D_MOD_PLANES_STATIC: case L4D_MOD_PLANES_DYNAMIC:
+      for (uint32_t s = 0; s < cfg->n_plane_scales; ++s)
+        for (int ci = 0; ci < 6; ++ci)
+          if (!grads->planes[s][ci]) return l4d_fail(L4D_EINVAL, "null plane gradient buffer");
+      break;
+    default: {       // dynamic hash: the slices the call reaches
+      const bool all = module == L4D_MOD_HASH_DYNAMIC;
+      for (uint32_t p = 0; p < 3; ++p) {
+        const bool used = all || module == L4D_MOD_HASH_T0 + p || module == L4D_MOD_HASH_SLICE0 + p;
+        if (!used) continue;
+        const bool slice_mod = module >= L4D_MOD_HASH_SLICE0;
+        if (!grads->hash_dynamic[p][slice_mod ? slice : A.q.slice_lo] || (!slice_mod && !grads->hash_dynamic[p][A.q.slice_hi]))
+          return l4d_fail(L4D_EINVAL, "null hash_dynamic gradient buffer");
+      }
+    }
+  }
+  if (n == 0) return L4D_OK;
+  build_grads(cfg, grads, grad_work, A.G);
+  A.g_out = g_out; A.g_x = g_x;
+  const bool flow = module == L4D_MOD_FLOW;
+  const size_t smem = flow ? (80 * L4D_NT + 2 * L4D_NT * L4D_TILE_LD) * sizeof(float) : 0;
+  int grid;
+  rc = grid_for(k_module_bwd<L4D_NT>, L4D_NT, smem, (n + L4D_NT - 1) / L4D_NT, grid);
+  if (rc != L4D_OK) return rc;
+  ++g_launches; k_module_bwd<L4D_NT><<<grid, L4D_NT, smem, (cudaStream_t)stream>>>(A);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+static int mlp_check(const L4DConfig* cfg, const void* staged, uint32_t net, const float* in, uint32_t n, MlpArgs& A) {
+  int rc = check_config(cfg);
+  if (rc != L4D_OK) return rc;
+  if (!staged || !in) return l4d_fail(L4D_EINVAL, "null pointer");
+  if (misaligned4(in)) return l4d_fail(L4D_EINVAL, "misaligned pointer");
+  if (n > (1u << 31)) return l4d_fail(L4D_EINVAL, "n > 2^31");
+  if (net > L4D_NET_INTENSITY) return l4d_fail(L4D_EINVAL, "unknown net id");
+  memset(&A, 0, sizeof(A));
+  build_model(cfg, staged, A.M);
+  A.net = net; A.in = in; A.n = n;
+  A.n_in = net == L4D_NET_SIGMA ? cfg->sigma_in_dim : cfg->attr_in_dim;
+  A.n_out = net == L4D_NET_SIGMA ? 16 : 1;
+  return L4D_OK;
+}
+
+extern "C" int l4d_mlp_forward(const L4DConfig* cfg, const void* staged, uint32_t net, const float* in, uint32_t n,
+                               float* out, void* stream) {
+  MlpArgs A;
+  int rc = mlp_check(cfg, staged, net, in, n, A);
+  if (rc != L4D_OK) return rc;
+  if (!out) return l4d_fail(L4D_EINVAL, "null pointer");
+  if (misaligned4(out)) return l4d_fail(L4D_EINVAL, "misaligned pointer");
+  if (n == 0) return L4D_OK;
+  A.out = out;
+  const size_t smem = 64 * L4D_NT * sizeof(float);
+  int grid;
+  rc = grid_for(k_mlp_fwd<L4D_NT>, L4D_NT, smem, (n + L4D_NT - 1) / L4D_NT, grid);
+  if (rc != L4D_OK) return rc;
+  ++g_launches; k_mlp_fwd<L4D_NT><<<grid, L4D_NT, smem, (cudaStream_t)stream>>>(A);
+  L4D_CUDA(cudaGetLastError());
+  return L4D_OK;
+}
+
+extern "C" int l4d_mlp_backward(const L4DConfig* cfg, const void* staged, uint32_t net, const float* in, uint32_t n,
+                                const float* g_out, float* g_in, const L4DMasterGrads* grads, void* grad_work,
+                                size_t grad_work_bytes, void* stream) {
+  MlpArgs A;
+  int rc = mlp_check(cfg, staged, net, in, n, A);
+  if (rc != L4D_OK) return rc;
+  if (!g_out || !grads || !grad_work) return l4d_fail(L4D_EINVAL, "null pointer");
+  if (misaligned4(g_out) || misaligned4(g_in) || misaligned4(grad_work)) return l4d_fail(L4D_EINVAL, "misaligned pointer");
+  if (grad_work_bytes < grad_work_layout(cfg).total) return l4d_fail(L4D_ESIZE, "grad_work buffer too small");
+  const float* master = net == L4D_NET_SIGMA ? grads->sigma_net : (net == L4D_NET_RAYDROP ? grads->raydrop_net : grads->intensity_net);
+  if (!master) return l4d_fail(L4D_EINVAL, "null network gradient buffer");
+  if (n == 0) return L4D_OK;
+  build_grads(cfg, grads, grad_work, A.G);
+  A.g_out = g_out; A.g_in = g_in;
+  const size_t smem = (64 * L4D_NT + 2 * L4D_NT * L4D_TILE_LD) * sizeof(float);
+  int grid;
+  rc = grid_for(k_mlp_bwd<L4D_NT>, L4D_NT, smem, (n + L4D_NT - 1) / L4D_NT, grid);
+  if (rc != L4D_OK) return rc;
+  ++g_launches; k_mlp_bwd<L4D_NT><<<grid, L4D_NT, smem, (cudaStream_t)stream>>>(A);
   L4D_CUDA(cudaGetLastError());
   return L4D_OK;
 }

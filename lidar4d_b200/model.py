@@ -17,6 +17,7 @@ from __future__ import annotations
 import ctypes as C
 import itertools
 import math
+import weakref
 from typing import Dict, List, Optional
 
 import numpy as np
@@ -24,19 +25,34 @@ import torch
 import torch.nn as nn
 
 from . import _capi
-from .geometry import FieldConfig, make_frame
+from .geometry import FieldConfig, make_frame, make_time_query
 
 
 # =============================================================================
 # parameter containers with the reference's module / parameter names
 # =============================================================================
-class _TcnnParams(nn.Module):
-    """Stands where a tcnn.Encoding / tcnn.Network stood: a flat fp32 `params`
-    vector and `n_output_dims` (hash_field.py:137-139, lidar4d.py:84,96,108)."""
+class _Submodule(nn.Module):
+    """A submodule of LiDAR4D that runs its own CUDA op: it reaches the owner's engine through a weak link that
+    LiDAR4D sets after construction (a registered back-reference would make the module tree cyclic)."""
 
-    def __init__(self, n_params: int, n_output_dims: int, init: str, **kw):
+    _owner_ref = None
+
+    def _owner(self) -> "LiDAR4D":
+        owner = self._owner_ref() if self._owner_ref is not None else None
+        if owner is None:
+            raise RuntimeError(f"{type(self).__name__} runs through the LiDAR4D that owns it; build it inside a LiDAR4D")
+        return owner
+
+
+class _TcnnParams(_Submodule):
+    """Stands where a tcnn.Encoding / tcnn.Network stood: a flat fp32 `params` vector and `n_output_dims`
+    (hash_field.py:137-139, lidar4d.py:84,96,108).  `kind` says which encoding or network it is, and thereby what its
+    forward runs: "hash_static", ("hash_slice", plane, slice), "flow_grid", "freq", "sigma", "raydrop", "intensity"."""
+
+    def __init__(self, n_params: int, n_output_dims: int, init: str, kind=None, **kw):
         super().__init__()
         self.n_output_dims = n_output_dims
+        self.kind = kind
         p = torch.empty(n_params)
         if init == "hash":
             p.uniform_(-1e-4, 1e-4)                      # tcnn grid init [tcnn-ext]
@@ -52,28 +68,80 @@ class _TcnnParams(nn.Module):
             pass
         self.params = nn.Parameter(p)
 
-    def forward(self, *a, **k):
-        raise RuntimeError("encoders/MLPs are fused into the render kernel; call LiDAR4D.render/run/flow/density")
+    def forward(self, x):
+        """tcnn semantics on x [N, in] (encodings: coordinates in [0, 1]) -> [N, n_output_dims] float32.  Networks pad
+        their input with ones to the network width and give dL/dx; encodings give no input gradient."""
+        owner = self._owner()
+        c = owner.cfg
+        k = self.kind
+        if k == "hash_static":
+            return _run_module(owner, "enc", _capi.MOD_HASH_STATIC, x, 3, 4 * c.n_levels_hash,
+                               ["hash_encoder.hash_static.params"], "hash_encoder.hash_static")
+        if isinstance(k, tuple) and k[0] == "hash_slice":
+            _, p, t = k
+            return _run_module(owner, "enc", _capi.MOD_HASH_SLICE0 + p, x, 2, 4 * c.n_levels_hash,
+                               [f"hash_encoder.hash_dynamic.{p}.hash_t.{t}.params"],
+                               f"hash_encoder.hash_dynamic[{p}].hash_t[{t}]", slice_=t)
+        if k == "flow_grid":
+            return _run_module(owner, "enc", _capi.MOD_FLOW_GRID, x, 3, 8 * c.flow_n_levels,
+                               ["flow_net.grid_enc.params"], "flow_net.grid_enc")
+        if k == "freq":
+            return _run_module(owner, "enc", _capi.MOD_FREQ, x, 3, c.view_dim, [], "view_encoder")
+        if k == "sigma":
+            return _run_module(owner, "mlp", _capi.NET_SIGMA, x, c.sigma_in_dim, 1 + c.geo_feat_dim,
+                               ["sigma_net.params"], "sigma_net", input_grad=True)
+        if k in ("raydrop", "intensity"):
+            net = _capi.NET_RAYDROP if k == "raydrop" else _capi.NET_INTENSITY
+            return _run_module(owner, "mlp", net, x, c.attr_in_dim, 1, [f"{k}_net.params"], f"{k}_net",
+                               input_grad=True)
+        raise RuntimeError(f"this _TcnnParams ({k!r}) has no forward")
 
 
-class _HashGridT(nn.Module):
-    def __init__(self, n_params, time_resolution, n_output_dims):
+class _HashGridT(_Submodule):
+    def __init__(self, n_params, time_resolution, n_output_dims, plane: int):
         super().__init__()
-        self.hash_t = nn.ModuleList([_TcnnParams(n_params, n_output_dims * 4, "hash") for _ in range(time_resolution)])
+        self.hash_t = nn.ModuleList([_TcnnParams(n_params, n_output_dims * 4, "hash", kind=("hash_slice", plane, s))
+                                     for s in range(time_resolution)])
         self.n_output_dims = n_output_dims
+        self.plane = plane
+
+    def forward(self, x, t):
+        """HashGridT.forward (hash_field.py:76-88): x [N,2] in [0,1], t a float or a one-element tensor -> [N, L]."""
+        owner = self._owner()
+        c = owner.cfg
+        return _run_module(owner, "enc", _capi.MOD_HASH_T0 + self.plane, x, 2, c.n_levels_hash,
+                           [f"hash_encoder.hash_dynamic.{self.plane}.hash_t.{s}.params" for s in range(c.time_resolution)],
+                           f"hash_encoder.hash_dynamic[{self.plane}]", t=t)
 
 
-class _HashGrid4D(nn.Module):
+class _HashGrid4D(_Submodule):
     def __init__(self, cfg: FieldConfig):
         super().__init__()
         gs = cfg.static_grid()
-        self.hash_static = _TcnnParams(gs.n_params, gs.n_output_dims, "hash")
+        self.hash_static = _TcnnParams(gs.n_params, gs.n_output_dims, "hash", kind="hash_static")
         self.hash_dynamic = nn.ModuleList([
-            _HashGridT(cfg.dynamic_grid(p).n_params, cfg.time_resolution, cfg.hash_dynamic_dim // 3) for p in range(3)])
+            _HashGridT(cfg.dynamic_grid(p).n_params, cfg.time_resolution, cfg.hash_dynamic_dim // 3, p) for p in range(3)])
         self.n_output_dims = cfg.hash_static_dim + cfg.hash_dynamic_dim
 
+    def forward_static(self, x):
+        return self.hash_static(x)
 
-class _Planes4D(nn.Module):
+    def forward_dynamic(self, x, t):
+        """hash_field.py:146-158: x [N,3] in [0,1] -> cat(xy, xz, yz planes at t) [N, 3L]."""
+        owner = self._owner()
+        c = owner.cfg
+        names = [f"hash_encoder.hash_dynamic.{p}.hash_t.{s}.params" for p in range(3) for s in range(c.time_resolution)]
+        return _run_module(owner, "enc", _capi.MOD_HASH_DYNAMIC, x, 3, 3 * c.n_levels_hash, names,
+                           "hash_encoder.forward_dynamic", t=t)
+
+    def forward(self, x, t):
+        return [self.forward_static(x), self.forward_dynamic(x, t)]
+
+
+_STATIC_PLANES, _DYNAMIC_PLANES = (0, 1, 3), (2, 4, 5)
+
+
+class _Planes4D(_Submodule):
     """planes_field.py:144-190: ModuleList over scales of ParameterList over the 6 planes."""
 
     def __init__(self, cfg: FieldConfig):
@@ -93,16 +161,43 @@ class _Planes4D(nn.Module):
             self.planes.append(pl)
         self.n_output_dims = 2 * cfg.plane_dim
 
+    def _sample(self, xt, dynamic: bool):
+        owner = self._owner()
+        c = owner.cfg
+        names = [f"planes_encoder.planes.{s}.{ci}" for s in range(c.n_levels_plane)
+                 for ci in (_DYNAMIC_PLANES if dynamic else _STATIC_PLANES)]
+        return _run_module(owner, "enc", _capi.MOD_PLANES_DYNAMIC if dynamic else _capi.MOD_PLANES_STATIC, xt, 4,
+                           c.plane_dim, names, "planes_encoder", input_grad=True)
 
-class _FlowField(nn.Module):
+    def forward_static(self, xt):
+        """planes_field.py:198-209: xt [N,4] in [0,1] -> [N, 8S]; differentiable w.r.t. the planes and xt."""
+        return self._sample(xt, False)
+
+    def forward_dynamic(self, xt):
+        """planes_field.py:211-222: time planes at each row's own xt[:, 3]."""
+        return self._sample(xt, True)
+
+    def forward(self, xt):
+        return [self.forward_static(xt), self.forward_dynamic(xt)]
+
+
+class _FlowField(_Submodule):
     def __init__(self, cfg: FieldConfig):
         super().__init__()
         gf = cfg.flow_grid()
-        self.grid_enc = _TcnnParams(gf.n_params, gf.n_output_dims, "hash")
+        self.grid_enc = _TcnnParams(gf.n_params, gf.n_output_dims, "hash", kind="flow_grid")
         h = cfg.hidden_dim_flow
         self.mlp = nn.Sequential(nn.Linear(gf.n_output_dims // 4, h, bias=False), nn.ReLU(),
                                  nn.Linear(h, h, bias=False), nn.ReLU(), nn.Linear(h, 6, bias=False))
         torch.nn.init.normal_(self.mlp[-1].weight.data, 0, 0.001)     # flow_field.py:100
+
+    def forward(self, xt):
+        """flow_field.py:113-130: xt [N,4] in [0,1] -> flow [N,6].  The time of every row is xt[0,3] (as there), read
+        on the device.  Differentiable w.r.t. the grid and the three Linear weights, not w.r.t. xt."""
+        owner = self._owner()
+        return _run_module(owner, "enc", _capi.MOD_FLOW, xt, 4, 6,
+                           ["flow_net.grid_enc.params", "flow_net.mlp.0.weight", "flow_net.mlp.2.weight",
+                            "flow_net.mlp.4.weight"], "flow_net")
 
 
 # =============================================================================
@@ -136,6 +231,7 @@ class _Engine:
         self._stamp = None
         self._staged_grad_mode = None
         self._chk = None
+        self._chk_grad = None      # device checksum of the masters at grad-mode submodule calls (note_grad_content)
         self.stage_gen = 0         # bumped by every re-staging; forward records it, backward checks it
         self.static_params = False # True: skip the content check of no-grad calls (tight inference loops)
         self.flat_p = None
@@ -321,19 +417,28 @@ class _Engine:
             self._mtab = (base, tab)
         return self._mtab[1]
 
-    def ensure_staged(self):
+    def ensure_staged(self, across_grad_mode: bool = False):
         """Refresh the fp16 / channels-last / transposed working set when a master parameter changed.
         Change detection: autograd version counters (optimizer.step, load_state_dict) in grad mode; in no-grad mode
         additionally the CONTENT (one reduction + one 8-byte read), because torch_ema's copy_to()/restore()
         (runner.py:565-567,680,820) write through ``.data`` and leave the counters alone; and always when the grad mode
-        flipped since the last staging (eval -> train after ema.restore())."""
+        flipped since the last staging (eval -> train after ema.restore()).
+        across_grad_mode (submodule calls): a grad-mode forward written with the submodules makes some of its calls under
+        torch.no_grad() (lidar4d.py:160-161,169-170), and re-staging there would invalidate that forward's backward.  A
+        grad -> no-grad flip therefore keeps the working set when the masters' content equals what the grad-mode
+        submodule calls since the staging recorded (note_grad_content); without such a record, or with other content
+        (an EMA swap), it re-stages as above."""
         lib = self._lib()
         ts = self.tensors()
         reflat = self.ensure_flat(ts)
         grad_mode = torch.is_grad_enabled()
         stamp = tuple(t._version for t in ts.values())
-        need = (self.staged is None or reflat or stamp != self._stamp or self.staged.device != self.device()
-                or grad_mode != self._staged_grad_mode)
+        need = (self.staged is None or reflat or stamp != self._stamp or self.staged.device != self.device())
+        flip = grad_mode != self._staged_grad_mode
+        if (across_grad_mode and flip and not need and not grad_mode and self._chk_grad is not None
+                and self._checksum() == int(self._chk_grad)):
+            return
+        need = need or flip
         chk = None
         if not need and not grad_mode and not self.static_params:
             chk = self._checksum()
@@ -358,6 +463,13 @@ class _Engine:
                                          what, self.stream())
         _capi.check(lib, rc, "l4d_stage_params_ex")
         self.stage_gen += 1
+        self._chk_grad = None
+
+    def note_grad_content(self):
+        """Record (on the device, no host read) the masters' content of a grad-mode submodule call, once per staging:
+        ensure_staged(across_grad_mode=True) compares a later no-grad call against it."""
+        if self._chk_grad is None and self._staged_grad_mode:
+            self._chk_grad = self.flat_p.view(torch.int32).sum(dtype=torch.int64)
 
     def params_updated_by_optimizer(self, tables_staged: bool):
         """lidar4d_b200.optim.Adam wrote the parameter arena (and, fused, the fp16 tables): finish the refresh."""
@@ -657,6 +769,103 @@ class _AttributeFn(torch.autograd.Function):
         return (None, None, g_geo, None) + gw
 
 
+def _module_launch(eng: _Engine, kind: str, ident: int, q, slice_: int, x: torch.Tensor, out_dim: int):
+    lib = eng._lib()
+    n = x.shape[0]
+    out = torch.empty(n, out_dim, device=x.device)
+    if n:
+        with torch.cuda.device(x.device):
+            if kind == "enc":
+                rc = lib.l4d_encoder_forward(C.byref(eng.ccfg), eng.staged.data_ptr(), ident, C.byref(q), slice_,
+                                             x.data_ptr(), n, out.data_ptr(), eng.stream())
+            else:
+                rc = lib.l4d_mlp_forward(C.byref(eng.ccfg), eng.staged.data_ptr(), ident, x.data_ptr(), n, out.data_ptr(),
+                                         eng.stream())
+        _capi.check(lib, rc, f"l4d_{'encoder' if kind == 'enc' else 'mlp'}_forward")
+    return out
+
+
+# encoder modules whose backward accumulates into grad_work (planes, flow MLP), folded by l4d_unstage_grads
+_WORK_MODULES = (_capi.MOD_PLANES_STATIC, _capi.MOD_PLANES_DYNAMIC, _capi.MOD_FLOW)
+
+
+class _ModuleFn(torch.autograd.Function):
+    """One submodule call with a backward (l4d_encoder_backward / l4d_mlp_backward).  `params` are the module's own
+    parameters (named by `names`), with the two grad modes of _RenderFn; x gets dL/dx where the op gives one (planes,
+    networks).  Nothing is saved on the GPU: the backward recomputes from x."""
+
+    @staticmethod
+    def forward(ctx, eng: _Engine, kind, ident, q, slice_, out_dim, names, x, *params):
+        out = _module_launch(eng, kind, ident, q, slice_, x, out_dim)
+        ctx.eng, ctx.kind, ctx.ident, ctx.q, ctx.slice_, ctx.names = eng, kind, ident, q, slice_, names
+        ctx.stage_gen = eng.stage_gen
+        ctx.save_for_backward(x)
+        return out
+
+    @staticmethod
+    def backward(ctx, g_out):
+        eng = ctx.eng
+        lib = eng._lib()
+        eng.check_generation(ctx.stage_gen, "submodule backward")
+        (x,) = ctx.saved_tensors
+        n = x.shape[0]
+        g_out = g_out.contiguous().float()
+        want_x = ctx.needs_input_grad[7]
+        g_x = torch.zeros_like(x) if want_x else None
+        arena = eng.owner.grad_mode == "arena"
+        tab, views = (eng.attach_grads(), None) if arena else _scratch_grads(eng)
+        if n:
+            work = eng.work()
+            with torch.cuda.device(x.device):
+                if ctx.kind == "enc":
+                    rc = lib.l4d_encoder_backward(C.byref(eng.ccfg), eng.staged.data_ptr(), ctx.ident, C.byref(ctx.q),
+                                                  ctx.slice_, x.data_ptr(), n, g_out.data_ptr(),
+                                                  g_x.data_ptr() if want_x else None, C.byref(tab), work.data_ptr(),
+                                                  work.numel(), eng.stream())
+                else:
+                    rc = lib.l4d_mlp_backward(C.byref(eng.ccfg), eng.staged.data_ptr(), ctx.ident, x.data_ptr(), n,
+                                              g_out.data_ptr(), g_x.data_ptr() if want_x else None, C.byref(tab),
+                                              work.data_ptr(), work.numel(), eng.stream())
+                _capi.check(lib, rc, f"l4d_{'encoder' if ctx.kind == 'enc' else 'mlp'}_backward")
+                if ctx.kind == "mlp" or ctx.ident in _WORK_MODULES:     # the hash encodings write master gradients only
+                    rc = lib.l4d_unstage_grads(C.byref(eng.ccfg), work.data_ptr(), work.numel(), C.byref(tab),
+                                               eng.stream())
+                    _capi.check(lib, rc, "l4d_unstage_grads")
+        pg = (None,) * len(ctx.names) if arena else tuple(views[k] for k in ctx.names)
+        return (None,) * 7 + (g_x,) + pg
+
+
+def _run_module(owner: "LiDAR4D", kind: str, ident: int, x, in_dim: int, out_dim: int, names, label: str,
+                input_grad: bool = False, t=None, slice_: int = 0):
+    """Run one submodule op on x [..., in_dim] -> [N, out_dim].  In grad mode, with a parameter of `names` requiring grad
+    (or x, for ops with an input gradient), through _ModuleFn; otherwise one launch."""
+    eng = owner._engine
+    if not torch.is_tensor(x) or x.shape[-1] != in_dim:
+        raise ValueError(f"{label}: expected a tensor [N, {in_dim}], got {tuple(getattr(x, 'shape', ()))}")
+    eng._require_cuda(x)
+    grad = torch.is_grad_enabled()
+    if grad and x.requires_grad and not input_grad:
+        raise NotImplementedError(f"{label}: no gradient with respect to its input is implemented; detach the input "
+                                  "(the reference's own composition never needs it)")
+    q = _capi.L4DTimeQuery()
+    if t is not None:
+        if torch.is_tensor(t):
+            if t.numel() != 1:
+                raise ValueError(f"{label}: t must be a float or a one-element tensor")
+            t = float(t.reshape(-1)[0])     # one device->host read, the host branch of HashGridT.forward (hash_field.py:82)
+        q = _capi.make_time_query(make_time_query(t, owner.cfg.time_resolution))
+    eng.ensure_staged(across_grad_mode=True)
+    if grad:
+        eng.note_grad_content()
+    ts = eng.tensors()
+    params = [ts[k] for k in names]
+    x2 = x.reshape(-1, in_dim)
+    if grad and (any(p.requires_grad for p in params) or (input_grad and x.requires_grad)):
+        xin = x2.contiguous().float() if input_grad else x2.detach().contiguous().float()
+        return _ModuleFn.apply(eng, kind, ident, q, slice_, out_dim, tuple(names), xin, *params)
+    return _module_launch(eng, kind, ident, q, slice_, x2.detach().contiguous().float(), out_dim)
+
+
 # =============================================================================
 # public modules
 # =============================================================================
@@ -727,12 +936,14 @@ class LiDAR4D(LiDAR_Renderer):
 
         self.planes_encoder = _Planes4D(c)
         self.hash_encoder = _HashGrid4D(c)
-        self.view_encoder = _TcnnParams(0, c.view_dim, "empty")
+        self.view_encoder = _TcnnParams(0, c.view_dim, "empty", kind="freq")
         self.flow_net = _FlowField(c)
-        self.sigma_net = _TcnnParams(c.mlp_param_count(c.sigma_in_pad, 64, 1), 1 + geo_feat_dim, "mlp",
+        self.sigma_net = _TcnnParams(c.mlp_param_count(c.sigma_in_pad, 64, 1), 1 + geo_feat_dim, "mlp", kind="sigma",
                                      dims=[c.sigma_in_pad, 64, 16])
-        self.intensity_net = _TcnnParams(c.mlp_param_count(c.attr_in_pad, 64, 2), 1, "mlp", dims=[c.attr_in_pad, 64, 64, 16])
-        self.raydrop_net = _TcnnParams(c.mlp_param_count(c.attr_in_pad, 64, 2), 1, "mlp", dims=[c.attr_in_pad, 64, 64, 16])
+        self.intensity_net = _TcnnParams(c.mlp_param_count(c.attr_in_pad, 64, 2), 1, "mlp", kind="intensity",
+                                         dims=[c.attr_in_pad, 64, 64, 16])
+        self.raydrop_net = _TcnnParams(c.mlp_param_count(c.attr_in_pad, 64, 2), 1, "mlp", kind="raydrop",
+                                       dims=[c.attr_in_pad, 64, 64, 16])
         # U-Net ray-drop refinement is a per-image post-process outside the hot path (SURVEY.md 8(f) #3);
         # callers that need it pass the reference's module in (model/unet.py), its state_dict keys stay `unet.*`.
         self.unet = unet if unet is not None else nn.Identity()
@@ -748,6 +959,17 @@ class LiDAR4D(LiDAR_Renderer):
         self.jitter_seed = 0
         self._jitter_calls = 0
         self._engine = _Engine(self)
+        self._link_submodules()
+
+    def _link_submodules(self):
+        ref = weakref.ref(self)
+        for m in self.modules():
+            if isinstance(m, _Submodule):
+                m._owner_ref = ref
+
+    def __setstate__(self, state):            # copy.deepcopy / unpickling: the copies' submodules run through the copy
+        super().__setstate__(state)
+        self._link_submodules()
 
     # ---- precision / pipeline switches ------------------------------------------------------
     def set_mlp_fp16(self, on: bool = True):
