@@ -222,6 +222,37 @@ int    l4d_render_backward_ex(const L4DConfig* cfg, const void* staged, const L4
 /* The compositing backward of the tensor-core split pipeline alone (the first kernel l4d_render_backward runs there), on
  * the saved buffer of a training forward: afterwards feature columns 0..3 of the saved dL/dfeature hold dL/dsigma,
  * dL/da0, dL/da1 and the attribute mask (0 / 1) of every sample.  Tensor-core configurations only (L4D_EINVAL else). */
+/* --- the same forward / backward over rays of SEVERAL frames in one launch (a training batch drawn across frames).
+ *     Ray r of the launch belongs to frame frames[(first_ray_phase + r) / rays_per_frame]; the phase lets a launch start
+ *     in the middle of a frame's rays.  Every frame gets its own contracted tables in `saved`
+ *     (l4d_saved_bytes_frames(cfg, n_rays, n_steps, n_frames) bytes) and its own slice- / basis- / time-row-independent
+ *     accumulators in `grad_work` (l4d_grad_work_bytes_frames(cfg, n_frames) bytes, zero-filled once like the single-frame
+ *     buffer; the per-frame folds clear it again).  A ray's jitter stream is ray_offset + r, as for one frame, so a launch
+ *     over B frames of N rays renders what B single-frame launches with ray_offset + b * N render, bit for bit.
+ *     With n_frames = 1 the buffers and the results are those of l4d_render_forward / l4d_render_backward_ex, which are
+ *     this call with a one-frame table.  L4D_EINVAL: n_frames = 0 or > L4D_MAX_FRAMES, rays_per_frame = 0,
+ *     first_ray_phase >= rays_per_frame, or first_ray_phase + n_rays > n_frames * rays_per_frame.  The backward must be
+ *     called with the same table as its forward.  The *_bytes_frames functions return 0 on a bad n_frames. */
+#define L4D_MAX_FRAMES 16
+typedef struct L4DFrameTable {
+  uint32_t n_frames;           /* 1 .. L4D_MAX_FRAMES */
+  uint32_t rays_per_frame;
+  uint32_t first_ray_phase;    /* < rays_per_frame */
+  uint32_t reserved;
+  L4DFrame frames[L4D_MAX_FRAMES];
+} L4DFrameTable;
+size_t l4d_saved_bytes_frames(const L4DConfig* cfg, uint32_t n_rays, uint32_t n_steps, uint32_t n_frames);
+size_t l4d_grad_work_bytes_frames(const L4DConfig* cfg, uint32_t n_frames);
+int    l4d_render_forward_frames(const L4DConfig* cfg, const void* staged, const L4DFrameTable* frames,
+                                 const L4DRays* rays, float* depth, float* image, float* wsum,
+                                 float* weights_or_null, float* zvals_or_null,
+                                 void* saved_or_null, size_t saved_bytes, void* stream);
+int    l4d_render_backward_frames(const L4DConfig* cfg, const void* staged, const L4DFrameTable* frames,
+                                  const L4DRays* rays, const void* saved, size_t saved_bytes,
+                                  const float* g_depth, const float* g_image,
+                                  const float* g_wsum_or_null, const float* g_weights_or_null,
+                                  const L4DMasterGrads* grads, void* grad_work, size_t grad_work_bytes,
+                                  void* ev_hash_done_or_null, void* stream);
 int    l4d_composite_backward(const L4DConfig* cfg, const L4DRays* rays, void* saved, size_t saved_bytes,
                               const float* g_depth, const float* g_image,
                               const float* g_wsum_or_null, const float* g_weights_or_null, void* stream);

@@ -13,6 +13,7 @@ from .geometry import FieldConfig, FrameConstants, GridGeometry, TimeQuery
 MAX_LEVELS = 16
 MAX_PLANE_SCALES = 4
 MAX_TIME_SLICES = 16
+MAX_FRAMES = 16                         # L4D_MAX_FRAMES: frames of one multi-frame render launch
 ABI_VERSION = 1
 STAGE_TABLES, STAGE_SMALL = 1, 2        # l4d_stage_params_ex `what`
 ADAM_CHUNK, ADAM_MAX_SEGMENTS = 1024, 64
@@ -49,6 +50,11 @@ class L4DFrame(C.Structure):
     _fields_ = [("time", C.c_float), ("frame_idx", C.c_uint32), ("has_fwd", C.c_uint32),
                 ("has_bwd", C.c_uint32), ("cur", L4DTimeQuery), ("fwd", L4DTimeQuery),
                 ("bwd", L4DTimeQuery), ("flow_basis", C.c_float * 4)]
+
+
+class L4DFrameTable(C.Structure):
+    _fields_ = [("n_frames", C.c_uint32), ("rays_per_frame", C.c_uint32), ("first_ray_phase", C.c_uint32),
+                ("reserved", C.c_uint32), ("frames", L4DFrame * MAX_FRAMES)]
 
 
 class L4DMasterParams(C.Structure):
@@ -136,6 +142,18 @@ def _tq(q: Optional[TimeQuery]) -> L4DTimeQuery:
     return s
 
 
+def make_frame_table(frames, rays_per_frame: int, first_ray_phase: int = 0) -> L4DFrameTable:
+    """L4DFrameTable over `frames` (L4DFrame structs, at most MAX_FRAMES): ray r of a launch belongs to
+    frames[(first_ray_phase + r) // rays_per_frame]."""
+    if not 1 <= len(frames) <= MAX_FRAMES:
+        raise ValueError(f"a frame table holds 1 to {MAX_FRAMES} frames, got {len(frames)}")
+    t = L4DFrameTable()
+    t.n_frames, t.rays_per_frame, t.first_ray_phase = len(frames), int(rays_per_frame), int(first_ray_phase)
+    for i, f in enumerate(frames):
+        t.frames[i] = f
+    return t
+
+
 def make_frame_struct(fr: FrameConstants) -> L4DFrame:
     f = L4DFrame()
     f.time = float(fr.time)
@@ -172,6 +190,7 @@ EXPORTS = [
     "l4d_box_mask", "l4d_bce_loss_work_bytes", "l4d_bce_loss", "l4d_bce_loss_backward",
     "l4d_composite_backward",
     "l4d_main_loss_work_bytes", "l4d_main_loss", "l4d_main_loss_backward", "l4d_main_eval_loss",
+    "l4d_saved_bytes_frames", "l4d_grad_work_bytes_frames", "l4d_render_forward_frames", "l4d_render_backward_frames",
 ]
 SWEEP_SIM, SWEEP_TEST, SWEEP_EVAL = 0, 1, 2     # L4D_SWEEP_* layouts of l4d_sweep_images
 SWEEP_F32, SWEEP_F16 = 0, 1                     # L4D_SWEEP_* ray-drop dtypes
@@ -208,6 +227,16 @@ def declare(lib, prefix: str = "l4d_", host_sim: bool = False):
         lib.l4d_render_backward_ex.argtypes = [P(L4DConfig), V, P(L4DFrame), P(L4DRays), V, SZ, V, V, V, V,
                                                P(L4DMasterGrads), V, SZ, V, V]
         lib.l4d_render_backward_ex.restype = C.c_int
+        # several frames in one launch: the same arguments with an L4DFrameTable instead of one L4DFrame
+        lib.l4d_saved_bytes_frames.argtypes = [P(L4DConfig), U32, U32, U32]
+        lib.l4d_saved_bytes_frames.restype = SZ
+        lib.l4d_grad_work_bytes_frames.argtypes = [P(L4DConfig), U32]
+        lib.l4d_grad_work_bytes_frames.restype = SZ
+        lib.l4d_render_forward_frames.argtypes = [P(L4DConfig), V, P(L4DFrameTable), P(L4DRays), V, V, V, V, V, V, SZ, V]
+        lib.l4d_render_forward_frames.restype = C.c_int
+        lib.l4d_render_backward_frames.argtypes = [P(L4DConfig), V, P(L4DFrameTable), P(L4DRays), V, SZ, V, V, V, V,
+                                                   P(L4DMasterGrads), V, SZ, V, V]
+        lib.l4d_render_backward_frames.restype = C.c_int
         # the tensor-core pipeline's compositing backward alone (per-sample dL/dsigma, dL/da, mask -> saved dL/dfeature)
         lib.l4d_composite_backward.argtypes = [P(L4DConfig), P(L4DRays), V, SZ, V, V, V, V, V]
         lib.l4d_composite_backward.restype = C.c_int

@@ -258,9 +258,10 @@ L4D_WARP_FN void l4d_plane_scatter_warp_t(float* G, int W, const Bilerp& b, cons
   }
 }
 // gradient rows of the contracted time planes (DevGrads::pl_rows): the same run sums, and the tail lane only issues the two
-// texels of the row - the time-row weights are applied once per launch by k_fold_planes
-L4D_WARP_FN void l4d_row_scatter_warp(float* Grow, const Bilerp& b, const float g[8]) {
-  const WarpRuns r = l4d_warp_runs(b.x0);
+// texels of the row - the time-row weights are applied once per frame by k_fold_planes.  seg: the lane's frame in the launch
+// (lanes of different frames write different rows and never share a run; rows are far shorter than 2^16 texels)
+L4D_WARP_FN void l4d_row_scatter_warp(float* Grow, const Bilerp& b, const float g[8], int seg = 0) {
+  const WarpRuns r = l4d_warp_runs(b.x0 + (seg << 16));
   float s0[8], s1[8];
 #pragma unroll
   for (int c = 0; c < 8; ++c) { s0[c] = g[c] * b.wx0; s1[c] = g[c] * b.wx1; }
@@ -420,9 +421,9 @@ L4D_WARP_FN void l4d_static_vertex_scatter_warp(float* gbase, const uint32_t (&i
 
 // sink of a contracted time-plane row
 template <bool WARP_AGG>
-L4D_HD void l4d_row_sink(float* Grow, const Bilerp& b, const float g[8]) {
+L4D_HD void l4d_row_sink(float* Grow, const Bilerp& b, const float g[8], int seg = 0) {
 #if defined(__CUDA_ARCH__)
-  if (WARP_AGG) { l4d_row_scatter_warp(Grow, b, g); return; }
+  if (WARP_AGG) { l4d_row_scatter_warp(Grow, b, g, seg); return; }
 #endif
   l4d_row_scatter(Grow, b, g);
 }
@@ -463,7 +464,8 @@ struct DynHashCursor {
 // vertex over its run of lanes (l4d_vertex_sum) before it reduces.  seg: the lane's ray.
 template <bool WARP_AGG, class DF>
 L4D_HD void l4d_bw_dynhash_slice(const DevModel& M, const L4DFrame& F, const DevGrads& G, float x, float y, float z, float wc,
-                                 const DF& l4d_dfeat_fn, int row_hash_d, DynHashCursor& cur, int n, int seg, bool active) {
+                                 const DF& l4d_dfeat_fn, int row_hash_d, DynHashCursor& cur, int n, int seg, bool active,
+                                 size_t comb_off = 0) {
   if (!WARP_AGG && !active) return;
   const int L = (int)M.gs.n_levels;
   const bool quads = (L & 3) == 0;             // rows of a plane start on a multiple of 4: one 16-byte load per 4 levels
@@ -479,6 +481,7 @@ L4D_HD void l4d_bw_dynhash_slice(const DevModel& M, const L4DFrame& F, const Dev
     const float d = wc * (quads ? dsel : l4d_dfeat_fn(row_hash_d + p * L + l));
     float* gcomb = G.hd_comb[p];
     if (gcomb) {
+      gcomb += comb_off;
       // comb[entry] accumulates w_corner * d: ONE float per entry (the four features of an entry get basis[k] times it,
       // and the slice weights, in k_fold_dynamic).  The two x-corners of a cell are neighbours in the table (index =
       // cx ^ h(cy) or cx + cy * res) and fall into the same aligned quad of entries three times out of four: they go out
@@ -541,7 +544,8 @@ L4D_HD void l4d_bw_dynhash_slice(const DevModel& M, const L4DFrame& F, const Dev
 // scatter dL/dfeature through the encoders of one sample at (x,y,z) with its flow; dflow[6] out
 template <bool WARP_AGG, class DF, bool STATIC_HASH = true, bool ROWS = false>
 L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrads& G, float x, float y, float z,
-                             const float* flow, const DF& l4d_dfeat_fn, float (&dflow)[6], bool active, int seg = 0);
+                             const float* flow, const DF& l4d_dfeat_fn, float (&dflow)[6], bool active, int seg = 0,
+                             uint32_t frame = 0, size_t con_off = 0, size_t comb_off = 0);
 
 template <bool ROWS = false>
 L4D_HD void l4d_bw_scatter(const DevModel& M, const L4DFrame& F, const DevGrads& G, BwSample& s) {
@@ -554,10 +558,13 @@ L4D_HD void l4d_bw_scatter(const DevModel& M, const L4DFrame& F, const DevGrads&
 
 // ROWS: time planes are sampled from DevModel::pl_con and their gradients go to DevGrads::pl_rows (both must be set)
 // WARP_AGG: every lane of the warp must call (lanes without a sample pass active=false and a
-// provider that returns 0; they take part in the plane aggregation with zero contributions); seg: the sample's ray
+// provider that returns 0; they take part in the plane aggregation with zero contributions); seg: the sample's ray.
+// frame / con_off / comb_off: the sample's frame in a multi-frame launch and the float offsets of that frame's contracted
+// tables (DevModel::hd_con, pl_con) and accumulators (DevGrads::hd_comb, pl_rows) from the launch's first ones.
 template <bool WARP_AGG, class DF, bool STATIC_HASH, bool ROWS>
 L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrads& G, float x, float y, float z,
-                             const float* flow, const DF& l4d_dfeat_fn, float (&dflow)[6], bool active, int seg) {
+                             const float* flow, const DF& l4d_dfeat_fn, float (&dflow)[6], bool active, int seg,
+                             uint32_t frame, size_t con_off, size_t comb_off) {
 #pragma unroll
   for (int k = 0; k < 6; ++k) dflow[k] = 0.f;
   const int nS = (int)M.n_scales;
@@ -603,7 +610,13 @@ L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrad
 #pragma unroll 1
       for (int qi = 0; qi < 3; ++qi) {
         const float wq = qi == 0 ? wc : (qi == 1 ? wf : wb);
+        // the warp sinks need every lane: a query is skipped when no lane of the warp has it (lanes of a frame without
+        // that neighbour then take part with zero contributions; their frame has no contracted row for it to read)
+#if defined(__CUDA_ARCH__)
+        if (WARP_AGG ? !__any_sync(0xffffffffu, wq != 0.f) : wq == 0.f) continue;
+#else
         if (wq == 0.f) continue;
+#endif
         const float q0 = qi == 0 ? x : (qi == 1 ? xf0 : xw0);
         const float q1 = qi == 0 ? y : (qi == 1 ? xf1 : xw1);
         const float q2 = qi == 0 ? z : (qi == 1 ? xf2 : xw2);
@@ -612,10 +625,13 @@ L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrad
         Bilerp b0 = l4d_bilerp(q0, R, tau, T), b1 = l4d_bilerp(q1, R, tau, T), b2 = l4d_bilerp(q2, R, tau, T);
         // rows: the forward's contracted time planes (2 texels per sample) and their gradient rows, when the launch has them
         constexpr bool rows = ROWS;       // (a template parameter: the kernel is large, keep the other path out of it)
-        if (rows) {
-          l4d_row_sample<true>(M.pl_con[sc][0][qi], b0, v0, x0);
-          l4d_row_sample<true>(M.pl_con[sc][1][qi], b1, v1, x1);
-          l4d_row_sample<true>(M.pl_con[sc][2][qi], b2, v2, x2);
+        if (rows && wq == 0.f) {
+#pragma unroll
+          for (int c = 0; c < 8; ++c) v0[c] = v1[c] = v2[c] = x0[c] = x1[c] = x2[c] = 0.f;
+        } else if (rows) {
+          l4d_row_sample<true>(M.pl_con[sc][0][qi] + con_off, b0, v0, x0);
+          l4d_row_sample<true>(M.pl_con[sc][1][qi] + con_off, b1, v1, x1);
+          l4d_row_sample<true>(M.pl_con[sc][2][qi] + con_off, b2, v2, x2);
         } else {
           l4d_plane_sample<true>(M.planes[sc][2], R, b0, v0, x0);
           l4d_plane_sample<true>(M.planes[sc][4], R, b1, v1, x1);
@@ -624,13 +640,13 @@ L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrad
         float c0 = 0.f, c1 = 0.f, c2 = 0.f;
 #pragma unroll
         for (int c = 0; c < 8; ++c) { g[c] = wq * d[c] * v1[c] * v2[c]; c0 = fmaf(g[c], x0[c], c0); }
-        if (rows) l4d_row_sink<WARP_AGG>(G.pl_rows[sc][0][qi], b0, g); else l4d_plane_sink<WARP_AGG>(G.planes_cl[sc][2], R, b0, g, true);
+        if (rows) l4d_row_sink<WARP_AGG>(G.pl_rows[sc][0][qi] + comb_off, b0, g, (int)frame); else l4d_plane_sink<WARP_AGG>(G.planes_cl[sc][2], R, b0, g, true);
 #pragma unroll
         for (int c = 0; c < 8; ++c) { g[c] = wq * d[c] * v0[c] * v2[c]; c1 = fmaf(g[c], x1[c], c1); }
-        if (rows) l4d_row_sink<WARP_AGG>(G.pl_rows[sc][1][qi], b1, g); else l4d_plane_sink<WARP_AGG>(G.planes_cl[sc][4], R, b1, g, true);
+        if (rows) l4d_row_sink<WARP_AGG>(G.pl_rows[sc][1][qi] + comb_off, b1, g, (int)frame); else l4d_plane_sink<WARP_AGG>(G.planes_cl[sc][4], R, b1, g, true);
 #pragma unroll
         for (int c = 0; c < 8; ++c) { g[c] = wq * d[c] * v0[c] * v1[c]; c2 = fmaf(g[c], x2[c], c2); }
-        if (rows) l4d_row_sink<WARP_AGG>(G.pl_rows[sc][2][qi], b2, g); else l4d_plane_sink<WARP_AGG>(G.planes_cl[sc][5], R, b2, g, true);
+        if (rows) l4d_row_sink<WARP_AGG>(G.pl_rows[sc][2][qi] + comb_off, b2, g, (int)frame); else l4d_plane_sink<WARP_AGG>(G.planes_cl[sc][5], R, b2, g, true);
         if (qi == 1) { dflow[0] += c0; dflow[1] += c1; dflow[2] += c2; }
         if (qi == 2) { dflow[3] += c0; dflow[4] += c1; dflow[5] += c2; }
       }
@@ -652,7 +668,7 @@ L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrad
   }
 
   // dynamic hash
-  l4d_bw_dynhash_slice<WARP_AGG>(M, F, G, x, y, z, wc, l4d_dfeat_fn, row_hash_d, hc, 3 * L, seg, active);
+  l4d_bw_dynhash_slice<WARP_AGG>(M, F, G, x, y, z, wc, l4d_dfeat_fn, row_hash_d, hc, 3 * L, seg, active, comb_off);
 }
 
 // ---- B5: flow MLP backprop.  g[6] = dL/dflow of this sample. ----------------------------

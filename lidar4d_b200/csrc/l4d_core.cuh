@@ -46,7 +46,7 @@ static inline float l4d_opaque(float v) { volatile float t = v; return t; }
 
 // ---------------------------------------------------------------------------
 // device-side model description (passed by value as a __grid_constant__ kernel
-// parameter, < 4 KB together with the frame constants)
+// parameter, with the launch's frame table)
 // ---------------------------------------------------------------------------
 struct DevGrid {
   float    scale[L4D_MAX_LEVELS];
@@ -64,9 +64,9 @@ struct DevModel {
   uint32_t hd_slice_entries[3]; // entries per time slice
   // optional, per launch (split pipeline): the dynamic tables contracted with the frame's time constants, ONE fp32 per
   // entry and time query (cur, fwd, bwd): con[e] = sum_k basis[k] * (w_lo * T_lo[e][k] + w_hi * T_hi[e][k]).  Every sample
-  // of a launch shares the frame, and the feature is linear in the table, so k_contract_dynamic does this once per entry
+  // of a frame shares its time, and the feature is linear in the table, so k_contract_dynamic does this once per entry
   // instead of once per corner of every sample, and the gather reads 4 bytes per corner instead of a 16-byte pair record.
-  const float* hd_con[3][3];    // [plane][query][entries]; nullptr = gather from the pair records
+  const float* hd_con[3][3];    // [plane][query][entries] of the launch's first frame; nullptr = gather from the pair records
   // same idea for the three time planes (x,t) (y,t) (z,t) of every scale: the time coordinate of a query is a launch
   // constant, so its two plane rows are blended once (k_contract_planes) into ONE row [R][8] per (scale, plane, query) and a
   // sample reads 2 texels instead of 4.  Indexed [scale][0..2 = planes 2,4,5][query cur|fwd|bwd].
@@ -712,6 +712,14 @@ L4D_HD void l4d_emit(float (&acc)[L4D_H], const DevModel& M, float* xb, int xs, 
   if (ACC) l4d_layer64(acc, xb, xs, n, M.sig_w1t + (size_t)row0 * L4D_H);
 }
 
+// frame of ray `ray` of a launch (L4DFrameTable); a one-frame table needs no division.  MF = false: the kernel is the
+// compile-time one-frame specialisation (frame 0's constants then sit at fixed parameter offsets instead of being loaded
+// through a per-ray index, which raised the spills of the gather, the scatter and the fused forward)
+template <bool MF = true>
+L4D_HD uint32_t l4d_frame_of(const L4DFrameTable& T, uint32_t ray) {
+  return (!MF || T.n_frames == 1u) ? 0u : (T.first_ray_phase + ray) / T.rays_per_frame;
+}
+
 // weights of the neighbour aggregation 0.5*cur + 0.25*(fwd+bwd) with the
 // missing neighbour replaced by cur (lidar4d.py:155-176)
 L4D_HD void l4d_agg_weights(const L4DFrame& F, float& wc, float& wf, float& wb) {
@@ -722,9 +730,10 @@ L4D_HD void l4d_agg_weights(const L4DFrame& F, float& wc, float& wf, float& wb) 
 
 // all encoder features of one sample given its flow; order = cat([plane_s, plane_d, hash_s, hash_d]).
 // STATIC_HASH = false leaves out the static-hash rows: the split pipeline gathers them level-major (l4d_static_sweep, l4d_split.cuh).
+// con_off: floats from the launch's first contracted tables (DevModel::hd_con / pl_con) to those of the sample's frame.
 template <bool ACC, bool STATIC_HASH = true>
 L4D_HD void l4d_gather_features(const DevModel& M, const L4DFrame& F, float x, float y, float z, const float (&flow)[8],
-                                float* xb, int xs, const FeatSink& sink, float (&acc)[L4D_H]) {
+                                float* xb, int xs, const FeatSink& sink, float (&acc)[L4D_H], size_t con_off = 0) {
   const int nS = (int)M.n_scales;
   const int L = (int)M.gs.n_levels;
   const int row_plane_d = nS * 8;
@@ -767,9 +776,9 @@ L4D_HD void l4d_gather_features(const DevModel& M, const L4DFrame& F, float x, f
         float v0[8], v1[8], v2[8], dummy[8];
         Bilerp b0 = l4d_bilerp(q0, R, tau, T), b1 = l4d_bilerp(q1, R, tau, T), b2 = l4d_bilerp(q2, R, tau, T);
         if (M.pl_con[s][0][0]) {        // contracted rows of this launch (k_contract_planes)
-          l4d_row_sample<false>(M.pl_con[s][0][qi], b0, v0, dummy);
-          l4d_row_sample<false>(M.pl_con[s][1][qi], b1, v1, dummy);
-          l4d_row_sample<false>(M.pl_con[s][2][qi], b2, v2, dummy);
+          l4d_row_sample<false>(M.pl_con[s][0][qi] + con_off, b0, v0, dummy);
+          l4d_row_sample<false>(M.pl_con[s][1][qi] + con_off, b1, v1, dummy);
+          l4d_row_sample<false>(M.pl_con[s][2][qi] + con_off, b2, v2, dummy);
         } else {
           l4d_plane_sample<false>(M.planes[s][2], R, b0, v0, dummy);
           l4d_plane_sample<false>(M.planes[s][4], R, b1, v1, dummy);
@@ -804,9 +813,9 @@ L4D_HD void l4d_gather_features(const DevModel& M, const L4DFrame& F, float x, f
     if (con[0]) {        // contracted tables of this launch (k_contract_dynamic)
 #pragma unroll 1
       for (int l = 0; l < L; ++l) {
-        float v = wc * l4d_encode2_con(M.gd[p], con[0], l, ca, cb);
-        if (wf != 0.f) v = fmaf(wf, l4d_encode2_con(M.gd[p], con[1], l, fa, fb), v);
-        if (wb != 0.f) v = fmaf(wb, l4d_encode2_con(M.gd[p], con[2], l, ba, bb), v);
+        float v = wc * l4d_encode2_con(M.gd[p], con[0] + con_off, l, ca, cb);
+        if (wf != 0.f) v = fmaf(wf, l4d_encode2_con(M.gd[p], con[1] + con_off, l, fa, fb), v);
+        if (wb != 0.f) v = fmaf(wb, l4d_encode2_con(M.gd[p], con[2] + con_off, l, ba, bb), v);
         xb[l * xs] = v;
       }
     } else {

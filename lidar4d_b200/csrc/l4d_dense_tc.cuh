@@ -1086,12 +1086,12 @@ __global__ void __launch_bounds__(128, 4) k_fwd_flow_tc(const __grid_constant__ 
     const float x = l4d_x01(__ldg(A.rays_o + 3 * ray), __ldg(A.rays_d + 3 * ray), zj, M.bound);
     const float y = l4d_x01(__ldg(A.rays_o + 3 * ray + 1), __ldg(A.rays_d + 3 * ray + 1), zj, M.bound);
     const float z = l4d_x01(__ldg(A.rays_o + 3 * ray + 2), __ldg(A.rays_d + 3 * ray + 2), zj, M.bound);
+    const float* b = A.FT.frames[l4d_frame_of(A.FT, ray)].flow_basis;
     float fin[16];
 #pragma unroll
     for (int l = 0; l < 8; ++l) {
       float e[8];
       l4d_encode3_f8(M.gf, M.hf, l, x, y, z, e);
-      const float* b = A.F.flow_basis;
       fin[2 * l] = ((b[0] * e[0] + b[1] * e[2]) + b[2] * e[4]) + b[3] * e[6];
       fin[2 * l + 1] = ((b[0] * e[1] + b[1] * e[3]) + b[2] * e[5]) + b[3] * e[7];
     }

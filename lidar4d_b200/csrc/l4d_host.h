@@ -25,6 +25,7 @@ struct GradWorkLayout {
   size_t flo_w0t, flo_w1t, flo_w2;
   size_t hd_comb[3], hf_comb;
   size_t pl_rows;          // [query][scale][plane 2|4|5][R][8]
+  size_t comb_frame;       // bytes of one frame's hd_comb .. pl_rows block; frame f's block is at + f * comb_frame
   size_t total;
 };
 
@@ -93,7 +94,8 @@ static inline void point_time_rows(const L4DConfig* c, T* base, T* (&tab)[L4D_MA
       }
 }
 
-static inline GradWorkLayout grad_work_layout(const L4DConfig* c) {
+// n_frames: the per-frame accumulators (hd_comb, hf_comb, pl_rows) once per frame of a multi-frame launch, frame-major
+static inline GradWorkLayout grad_work_layout(const L4DConfig* c, uint32_t n_frames = 1) {
   GradWorkLayout L;
   size_t o = 0;
   auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
@@ -117,7 +119,8 @@ static inline GradWorkLayout grad_work_layout(const L4DConfig* c) {
   for (int p = 0; p < 3; ++p) L.hd_comb[p] = take((size_t)c->hash_dynamic[p].offset[c->hash_dynamic[p].n_levels] * f);
   L.hf_comb = take((size_t)c->flow.offset[c->flow.n_levels] * 2 * f);
   L.pl_rows = take(time_rows_floats(c) * f);
-  L.total = o;
+  L.comb_frame = o - L.hd_comb[0];
+  L.total = L.hd_comb[0] + (size_t)n_frames * L.comb_frame;
   return L;
 }
 
@@ -197,7 +200,7 @@ static inline void build_model(const L4DConfig* c, const void* staged, DevModel&
 }
 
 static inline void build_grads(const L4DConfig* c, const L4DMasterGrads* g, void* grad_work, DevGrads& G, bool comb = false) {
-  GradWorkLayout L = grad_work_layout(c);
+  GradWorkLayout L = grad_work_layout(c);      // frame 0's accumulators: the others follow at L.comb_frame strides
   char* b = reinterpret_cast<char*>(grad_work);
   memset(&G, 0, sizeof(G));
   G.hs = g->hash_static;
@@ -220,8 +223,9 @@ static inline void build_grads(const L4DConfig* c, const L4DMasterGrads* g, void
 
 #define L4D_NT 128
 #define L4D_BWD_SCRATCH_CTAS 1024
-struct SavedLayout { size_t feat, flow_in, sigma, attr, hidden, flow, dfeat, dflow, tstart, hd_con, pl_con, total; };
-static inline SavedLayout saved_layout(const L4DConfig* c, uint32_t n_rays, uint32_t S) {
+struct SavedLayout { size_t feat, flow_in, sigma, attr, hidden, flow, dfeat, dflow, tstart, hd_con, pl_con, con_frame, total; };
+// n_frames: the contracted tables (hd_con, pl_con) once per frame of a multi-frame launch, frame-major, con_frame bytes apart
+static inline SavedLayout saved_layout(const L4DConfig* c, uint32_t n_rays, uint32_t S, uint32_t n_frames = 1) {
   SavedLayout L;
   const size_t P = (size_t)n_rays * S;
   const size_t tiles = (size_t)n_rays * ((S + 127) / 128);
@@ -244,7 +248,8 @@ static inline SavedLayout saved_layout(const L4DConfig* c, uint32_t n_rays, uint
   for (int p = 0; p < 3; ++p) dyn_entries += c->hash_dynamic[p].offset[c->hash_dynamic[p].n_levels];
   L.hd_con = take(3 * dyn_entries * sizeof(float));
   L.pl_con = take(time_rows_floats(c) * sizeof(float));      // contracted time-plane rows (DevModel::pl_con)
-  L.total = o;
+  L.con_frame = o - L.hd_con;
+  L.total = L.hd_con + (size_t)n_frames * L.con_frame;
   return L;
 }
 // what l4d_density_forward_ex saves for l4d_density_backward on n explicit points: the Lagrange-contracted flow-MLP
@@ -266,7 +271,7 @@ static inline DensitySavedLayout density_saved_layout(const L4DConfig* c, uint32
 }
 
 // DevModel::hd_con (dynamic-hash tables) and ::pl_con (time-plane rows) inside the saved buffer of a launch (level offsets,
-// hence plane sizes, are multiples of 8 entries)
+// hence plane sizes, are multiples of 8 entries): those of the launch's first frame
 static inline void point_contracted(const L4DConfig* c, void* saved, uint32_t n_rays, uint32_t S, DevModel& M) {
   SavedLayout L = saved_layout(c, n_rays, S);
   float* b = reinterpret_cast<float*>(reinterpret_cast<char*>(saved) + L.hd_con);

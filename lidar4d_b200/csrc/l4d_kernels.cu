@@ -623,7 +623,7 @@ __device__ __forceinline__ float tile_colsum(const float* __restrict__ T) {
 // =============================================================================
 struct FwdArgs {
   DevModel M;
-  L4DFrame F;
+  L4DFrameTable FT;
   const float* rays_o;
   const float* rays_d;
   uint32_t n_rays, S, perturb;
@@ -633,7 +633,7 @@ struct FwdArgs {
   uint32_t train;
 };
 
-template <int NT>
+template <int NT, bool MF>
 __global__ void __launch_bounds__(NT) k_render_fwd(const __grid_constant__ FwdArgs A) {
   extern __shared__ __align__(16) float smem[];
   float* xbuf = smem;                 // [64][NT]
@@ -641,13 +641,13 @@ __global__ void __launch_bounds__(NT) k_render_fwd(const __grid_constant__ FwdAr
   float* s_cdir = s_enc + 80;         // [128]
   float* s_w = s_cdir + 128;          // [32]
   const DevModel& M = A.M;
-  const L4DFrame& F = A.F;
   const int tid = threadIdx.x;
   float* xb = xbuf + tid;
   const RaySampling rs = l4d_make_sampling(M.near_lidar, M.far_lidar, A.S, A.perturb, A.seed);
   const uint32_t S = A.S;
 
   for (uint32_t ray = blockIdx.x; ray < A.n_rays; ray += gridDim.x) {
+    const L4DFrame& F = A.FT.frames[l4d_frame_of<MF>(A.FT, ray)];
     const float ox = __ldg(A.rays_o + 3 * ray), oy = __ldg(A.rays_o + 3 * ray + 1), oz = __ldg(A.rays_o + 3 * ray + 2);
     const float dx = __ldg(A.rays_d + 3 * ray), dy = __ldg(A.rays_d + 3 * ray + 1), dz = __ldg(A.rays_d + 3 * ray + 2);
     __syncthreads();
@@ -709,7 +709,7 @@ __global__ void __launch_bounds__(NT) k_render_fwd(const __grid_constant__ FwdAr
 #define L4D_MAX_TILES 64
 struct BwdArgs {
   DevModel M;
-  L4DFrame F;
+  L4DFrameTable FT;
   DevGrads G;
   const float* rays_o;
   const float* rays_d;
@@ -731,7 +731,6 @@ __global__ void __launch_bounds__(NT) k_render_bwd(const __grid_constant__ BwdAr
   float* s_w = s_csum + 128;                      // [32]
   float* s_tstart = s_w + 32;                     // [L4D_MAX_TILES]
   const DevModel& M = A.M;
-  const L4DFrame& F = A.F;
   const DevGrads& G = A.G;
   const int tid = threadIdx.x;
   float* xb = xbuf + tid;
@@ -745,6 +744,7 @@ __global__ void __launch_bounds__(NT) k_render_bwd(const __grid_constant__ BwdAr
   const int n_chunks = (int)(M.sigma_in_pad + 63) / 64;
 
   for (uint32_t ray = blockIdx.x; ray < A.n_rays; ray += gridDim.x) {
+    const L4DFrame& F = A.FT.frames[l4d_frame_of(A.FT, ray)];
     const float ox = __ldg(A.rays_o + 3 * ray), oy = __ldg(A.rays_o + 3 * ray + 1), oz = __ldg(A.rays_o + 3 * ray + 2);
     const float dx = __ldg(A.rays_d + 3 * ray), dy = __ldg(A.rays_d + 3 * ray + 1), dz = __ldg(A.rays_d + 3 * ray + 2);
     const float gd = __ldg(A.g_depth + ray), gi0 = __ldg(A.g_image + 2 * ray), gi1 = __ldg(A.g_image + 2 * ray + 1);
@@ -1072,8 +1072,41 @@ static int check_n_steps(uint32_t n_steps) {
 }
 
 extern "C" size_t l4d_saved_bytes(const L4DConfig* cfg, uint32_t n_rays, uint32_t n_steps) {
-  if (check_config(cfg) != L4D_OK || check_n_steps(n_steps) != L4D_OK) return 0;
-  return saved_layout(cfg, n_rays, n_steps).total;
+  return l4d_saved_bytes_frames(cfg, n_rays, n_steps, 1);
+}
+
+static int check_n_frames(uint32_t n_frames) {
+  if (n_frames == 0 || n_frames > L4D_MAX_FRAMES) return l4d_fail(L4D_EINVAL, "n_frames out of range [1, L4D_MAX_FRAMES]");
+  return L4D_OK;
+}
+extern "C" size_t l4d_saved_bytes_frames(const L4DConfig* cfg, uint32_t n_rays, uint32_t n_steps, uint32_t n_frames) {
+  if (check_config(cfg) != L4D_OK || check_n_steps(n_steps) != L4D_OK || check_n_frames(n_frames) != L4D_OK) return 0;
+  return saved_layout(cfg, n_rays, n_steps, n_frames).total;
+}
+extern "C" size_t l4d_grad_work_bytes_frames(const L4DConfig* cfg, uint32_t n_frames) {
+  if (check_config(cfg) != L4D_OK || check_n_frames(n_frames) != L4D_OK) return 0;
+  return grad_work_layout(cfg, n_frames).total;
+}
+
+// a frame table must name a frame for every ray of the launch
+static int check_frames(const L4DFrameTable* T, uint32_t n_rays) {
+  if (!T) return l4d_fail(L4D_EINVAL, "null frame table");
+  int rc = check_n_frames(T->n_frames);
+  if (rc != L4D_OK) return rc;
+  if (T->rays_per_frame == 0) return l4d_fail(L4D_EINVAL, "rays_per_frame is 0");
+  if (T->first_ray_phase >= T->rays_per_frame) return l4d_fail(L4D_EINVAL, "first_ray_phase >= rays_per_frame");
+  if ((uint64_t)T->first_ray_phase + n_rays > (uint64_t)T->n_frames * T->rays_per_frame)
+    return l4d_fail(L4D_EINVAL, "the frame table does not cover n_rays");
+  return L4D_OK;
+}
+// the one-frame table of the single-frame entry points
+static L4DFrameTable one_frame(const L4DFrame* frame, uint32_t n_rays) {
+  L4DFrameTable T;
+  memset(&T, 0, sizeof(T));
+  T.n_frames = 1;
+  T.rays_per_frame = n_rays > 0 ? n_rays : 1;
+  T.frames[0] = *frame;
+  return T;
 }
 
 static int check_rays(const L4DRays* r) {
@@ -1128,11 +1161,16 @@ static int grid_for(K kernel, int nt, size_t smem, uint32_t work, int& grid, int
   return L4D_OK;
 }
 
-static void fill_split(SplitArgs& A, const L4DConfig* cfg, const void* staged, const L4DFrame* frame, const L4DRays* rays,
+// the frame table travels in the kernel parameter block (no copy, no sync): it needs the large parameter space of CUDA 12.1+
+static_assert(sizeof(SplitArgs) <= 32764 && sizeof(FwdArgs) <= 32764 && sizeof(BwdArgs) <= 32764, "kernel parameter limit");
+
+static void fill_split(SplitArgs& A, const L4DConfig* cfg, const void* staged, const L4DFrameTable* frames, const L4DRays* rays,
                        void* saved) {
   memset(&A, 0, sizeof(A));
   build_model(cfg, staged, A.M);
-  A.F = *frame;
+  A.FT = *frames;
+  A.con_fstride = saved_layout(cfg, rays->n_rays, rays->n_steps).con_frame / sizeof(float);
+  A.comb_fstride = grad_work_layout(cfg).comb_frame / sizeof(float);
   A.rays_o = rays->rays_o; A.rays_d = rays->rays_d;
   A.n_rays = rays->n_rays; A.S = rays->n_steps; A.perturb = rays->perturb;
   A.seed = rays->seed; A.ray_offset = rays->ray_offset;
@@ -1196,21 +1234,34 @@ extern "C" int l4d_composite_backward(const L4DConfig* cfg, const L4DRays* rays,
 extern "C" int l4d_render_forward(const L4DConfig* cfg, const void* staged, const L4DFrame* frame, const L4DRays* rays,
                                   float* depth, float* image, float* wsum, float* weights, float* zvals, void* saved,
                                   size_t saved_bytes, void* stream) {
+  L4DFrameTable T;
+  const bool ok = frame && rays;
+  if (ok) T = one_frame(frame, rays->n_rays);
+  return l4d_render_forward_frames(cfg, staged, ok ? &T : nullptr, rays, depth, image, wsum, weights, zvals, saved, saved_bytes, stream);
+}
+
+extern "C" int l4d_render_forward_frames(const L4DConfig* cfg, const void* staged, const L4DFrameTable* frames,
+                                         const L4DRays* rays, float* depth, float* image, float* wsum, float* weights,
+                                         float* zvals, void* saved, size_t saved_bytes, void* stream) {
   int rc = check_config(cfg);
   if (rc != L4D_OK) return rc;
   rc = check_rays(rays);
   if (rc != L4D_OK) return rc;
-  if (!staged || !frame || !depth || !image || !wsum) return l4d_fail(L4D_EINVAL, "null pointer");
+  if (!staged || !frames || !depth || !image || !wsum) return l4d_fail(L4D_EINVAL, "null pointer");
+  rc = check_frames(frames, rays->n_rays);
+  if (rc != L4D_OK) return rc;
   if (rays->n_rays == 0) return L4D_OK;
-  if (saved && saved_bytes < saved_layout(cfg, rays->n_rays, rays->n_steps).total) return l4d_fail(L4D_ESIZE, "saved buffer too small");
+  if (saved && saved_bytes < saved_layout(cfg, rays->n_rays, rays->n_steps, frames->n_frames).total)
+    return l4d_fail(L4D_ESIZE, "saved buffer too small");
   const bool fused = (rays->reserved & L4D_FLAG_FUSED) || !saved;
+  const bool mf = frames->n_frames > 1;
   cudaStream_t st = (cudaStream_t)stream;
   prof_mark(st, "begin");
   if (fused) {
     FwdArgs A;
     memset(&A, 0, sizeof(A));
     build_model(cfg, staged, A.M);
-    A.F = *frame;
+    A.FT = *frames;
     A.rays_o = rays->rays_o; A.rays_d = rays->rays_d;
     A.n_rays = rays->n_rays; A.S = rays->n_steps; A.perturb = rays->perturb;
     A.seed = rays->seed; A.ray_offset = rays->ray_offset;
@@ -1219,48 +1270,53 @@ extern "C" int l4d_render_forward(const L4DConfig* cfg, const void* staged, cons
     if (saved) A.sv = saved_view(cfg, saved, rays->n_rays, rays->n_steps);
     const size_t smem = (64 * L4D_NT + 80 + 128 + 32) * sizeof(float);
     int grid;
-    rc = grid_for(k_render_fwd<L4D_NT>, L4D_NT, smem, rays->n_rays, grid);
+    auto kernel = mf ? k_render_fwd<L4D_NT, true> : k_render_fwd<L4D_NT, false>;
+    rc = grid_for(kernel, L4D_NT, smem, rays->n_rays, grid);
     if (rc != L4D_OK) return rc;
-    ++g_launches; k_render_fwd<L4D_NT><<<grid, L4D_NT, smem, st>>>(A);
+    ++g_launches; kernel<<<grid, L4D_NT, smem, st>>>(A);
     prof_mark(st, "k_render_fwd");
     L4D_CUDA(cudaGetLastError());
     return L4D_OK;
   }
   SplitArgs A;
-  fill_split(A, cfg, staged, frame, rays, saved);
+  fill_split(A, cfg, staged, frames, rays, saved);
   A.depth = depth; A.image = image; A.wsum = wsum; A.weights = weights; A.zvals = zvals;
   A.train = 1u;
   const size_t P = (size_t)rays->n_rays * rays->n_steps;
-  // per-launch contraction of the time-dependent encoders with the frame's constants: dynamic-hash tables
+  // contraction of the time-dependent encoders with each frame's constants, into that frame's dynamic-hash tables
   // (DevModel::hd_con) and time-plane rows (DevModel::pl_con)
   point_contracted(cfg, saved, rays->n_rays, rays->n_steps, A.M);
-  {
-    ContractArgs C;
-    memset(&C, 0, sizeof(C));
-    uint32_t nmax = 0;
-    for (int p = 0; p < 3; ++p) {
-      C.table[p] = reinterpret_cast<const uint4*>(A.M.hd[p]);
-      C.entries[p] = A.M.hd_slice_entries[p];
-      nmax = C.entries[p] > nmax ? C.entries[p] : nmax;
-      for (int q = 0; q < 3; ++q) C.con[p][q] = const_cast<float*>(A.M.hd_con[p][q]);
-    }
-    C.n_slices = cfg->time_resolution;
-    C.n_queries_mask = 1u | (frame->has_fwd ? 2u : 0u) | (frame->has_bwd ? 4u : 0u);
-    C.q[0] = frame->cur; C.q[1] = frame->fwd; C.q[2] = frame->bwd;
-    ++g_launches; k_contract_dynamic<<<dim3((unsigned)nblk(nmax), 3), 256, 0, st>>>(C);
-  }
-  {
-    TimeRowArgs T;
-    fill_time_rows(T, cfg, frame);
-    uint32_t rmax = 0;
-    for (uint32_t s2 = 0; s2 < cfg->n_plane_scales; ++s2) {
-      rmax = cfg->plane_res[s2] > rmax ? cfg->plane_res[s2] : rmax;
-      for (int t = 0; t < 3; ++t) {
-        T.plane[s2][t] = const_cast<float*>(A.M.planes[s2][t == 0 ? 2 : (t == 1 ? 4 : 5)]);
-        for (int q = 0; q < 3; ++q) T.row[s2][t][q] = const_cast<float*>(A.M.pl_con[s2][t][q]);
+  for (uint32_t f = 0; f < frames->n_frames; ++f) {
+    const L4DFrame* frame = &frames->frames[f];
+    const size_t off = f * A.con_fstride;
+    {
+      ContractArgs C;
+      memset(&C, 0, sizeof(C));
+      uint32_t nmax = 0;
+      for (int p = 0; p < 3; ++p) {
+        C.table[p] = reinterpret_cast<const uint4*>(A.M.hd[p]);
+        C.entries[p] = A.M.hd_slice_entries[p];
+        nmax = C.entries[p] > nmax ? C.entries[p] : nmax;
+        for (int q = 0; q < 3; ++q) C.con[p][q] = const_cast<float*>(A.M.hd_con[p][q]) + off;
       }
+      C.n_slices = cfg->time_resolution;
+      C.n_queries_mask = 1u | (frame->has_fwd ? 2u : 0u) | (frame->has_bwd ? 4u : 0u);
+      C.q[0] = frame->cur; C.q[1] = frame->fwd; C.q[2] = frame->bwd;
+      ++g_launches; k_contract_dynamic<<<dim3((unsigned)nblk(nmax), 3), 256, 0, st>>>(C);
     }
-    ++g_launches; k_contract_planes<<<dim3((unsigned)nblk((size_t)rmax * 8), 3 * cfg->n_plane_scales), 256, 0, st>>>(T);
+    {
+      TimeRowArgs T;
+      fill_time_rows(T, cfg, frame);
+      uint32_t rmax = 0;
+      for (uint32_t s2 = 0; s2 < cfg->n_plane_scales; ++s2) {
+        rmax = cfg->plane_res[s2] > rmax ? cfg->plane_res[s2] : rmax;
+        for (int t = 0; t < 3; ++t) {
+          T.plane[s2][t] = const_cast<float*>(A.M.planes[s2][t == 0 ? 2 : (t == 1 ? 4 : 5)]);
+          for (int q = 0; q < 3; ++q) T.row[s2][t][q] = const_cast<float*>(A.M.pl_con[s2][t][q]) + off;
+        }
+      }
+      ++g_launches; k_contract_planes<<<dim3((unsigned)nblk((size_t)rmax * 8), 3 * cfg->n_plane_scales), 256, 0, st>>>(T);
+    }
   }
   prof_mark(st, "k_contract");
   if (cfg->mlp_fp16) {
@@ -1276,21 +1332,24 @@ extern "C" int l4d_render_forward(const L4DConfig* cfg, const void* staged, cons
     int grid;
     if (use_tc_dense(cfg)) {
       const uint32_t work = rays->n_rays * A.sv.n_tiles;       // whole 128-row tiles
-      rc = grid_for(k_fwd_gather<L4D_NT, true, true>, L4D_NT, smem, work, grid);
+      auto kernel = mf ? k_fwd_gather<L4D_NT, true, true, true> : k_fwd_gather<L4D_NT, true, true, false>;
+      rc = grid_for(kernel, L4D_NT, smem, work, grid);
       if (rc != L4D_OK) return rc;
-      ++g_launches; k_fwd_gather<L4D_NT, true, true><<<grid, L4D_NT, smem, st>>>(A);
+      ++g_launches; kernel<<<grid, L4D_NT, smem, st>>>(A);
     } else {
-      rc = grid_for(k_fwd_gather<L4D_NT, true, false>, L4D_NT, smem, (uint32_t)((P + L4D_NT - 1) / L4D_NT), grid);
+      auto kernel = mf ? k_fwd_gather<L4D_NT, true, false, true> : k_fwd_gather<L4D_NT, true, false, false>;
+      rc = grid_for(kernel, L4D_NT, smem, (uint32_t)((P + L4D_NT - 1) / L4D_NT), grid);
       if (rc != L4D_OK) return rc;
-      ++g_launches; k_fwd_gather<L4D_NT, true, false><<<grid, L4D_NT, smem, st>>>(A);
+      ++g_launches; kernel<<<grid, L4D_NT, smem, st>>>(A);
     }
     prof_mark(st, "k_fwd_gather");
   } else {
     const size_t smem = 64 * L4D_NT * sizeof(float);
     int grid;
-    rc = grid_for(k_fwd_gather<L4D_NT, false, false>, L4D_NT, smem, (uint32_t)((P + L4D_NT - 1) / L4D_NT), grid);
+    auto kernel = mf ? k_fwd_gather<L4D_NT, false, false, true> : k_fwd_gather<L4D_NT, false, false, false>;
+    rc = grid_for(kernel, L4D_NT, smem, (uint32_t)((P + L4D_NT - 1) / L4D_NT), grid);
     if (rc != L4D_OK) return rc;
-    ++g_launches; k_fwd_gather<L4D_NT, false, false><<<grid, L4D_NT, smem, st>>>(A);
+    ++g_launches; kernel<<<grid, L4D_NT, smem, st>>>(A);
     prof_mark(st, "k_fwd_gather");
   }
   if (use_tc_dense(cfg)) {
@@ -1327,13 +1386,32 @@ extern "C" int l4d_render_backward_ex(const L4DConfig* cfg, const void* staged, 
                                       const void* saved, size_t saved_bytes, const float* g_depth, const float* g_image,
                                       const float* g_wsum, const float* g_weights, const L4DMasterGrads* grads,
                                       void* grad_work, size_t grad_work_bytes, void* ev_hash_done, void* stream) {
+  L4DFrameTable T;
+  const bool ok = frame && rays;
+  if (ok) T = one_frame(frame, rays->n_rays);
+  return l4d_render_backward_frames(cfg, staged, ok ? &T : nullptr, rays, saved, saved_bytes, g_depth, g_image, g_wsum, g_weights, grads,
+                                    grad_work, grad_work_bytes, ev_hash_done, stream);
+}
+
+extern "C" int l4d_render_backward_frames(const L4DConfig* cfg, const void* staged, const L4DFrameTable* frames,
+                                          const L4DRays* rays, const void* saved, size_t saved_bytes, const float* g_depth,
+                                          const float* g_image, const float* g_wsum, const float* g_weights,
+                                          const L4DMasterGrads* grads, void* grad_work, size_t grad_work_bytes,
+                                          void* ev_hash_done, void* stream) {
   int rc = check_config(cfg);
   if (rc != L4D_OK) return rc;
   rc = check_rays(rays);
   if (rc != L4D_OK) return rc;
-  if (!staged || !frame || !saved || !g_depth || !g_image || !grads || !grad_work) return l4d_fail(L4D_EINVAL, "null pointer");
-  if (saved_bytes < saved_layout(cfg, rays->n_rays, rays->n_steps).total) return l4d_fail(L4D_ESIZE, "saved buffer too small");
-  if (grad_work_bytes < grad_work_layout(cfg).total) return l4d_fail(L4D_ESIZE, "grad_work buffer too small");
+  if (!staged || !frames || !saved || !g_depth || !g_image || !grads || !grad_work) return l4d_fail(L4D_EINVAL, "null pointer");
+  rc = check_frames(frames, rays->n_rays);
+  if (rc != L4D_OK) return rc;
+  const bool fused = (rays->reserved & L4D_FLAG_FUSED) != 0;
+  const bool mf = frames->n_frames > 1;
+  if (saved_bytes < saved_layout(cfg, rays->n_rays, rays->n_steps, frames->n_frames).total)
+    return l4d_fail(L4D_ESIZE, "saved buffer too small");
+  // the single kernel accumulates straight into the slices: only the split pipeline has per-frame accumulators
+  if (grad_work_bytes < grad_work_layout(cfg, fused ? 1u : frames->n_frames).total)
+    return l4d_fail(L4D_ESIZE, "grad_work buffer too small");
   if (!grads->hash_static || !grads->flow_grid) return l4d_fail(L4D_EINVAL, "null hash gradient buffer");
   for (int p = 0; p < 3; ++p)
     for (uint32_t s = 0; s < cfg->time_resolution; ++s)
@@ -1341,9 +1419,9 @@ extern "C" int l4d_render_backward_ex(const L4DConfig* cfg, const void* staged, 
   if (rays->n_rays == 0) return L4D_OK;
   cudaStream_t st = (cudaStream_t)stream;
   prof_mark(st, "begin");
-  if (!(rays->reserved & L4D_FLAG_FUSED)) {
+  if (!fused) {
     SplitArgs A;
-    fill_split(A, cfg, staged, frame, rays, const_cast<void*>(saved));
+    fill_split(A, cfg, staged, frames, rays, const_cast<void*>(saved));
     build_grads(cfg, grads, grad_work, A.G, true);
     point_contracted(cfg, const_cast<void*>(saved), rays->n_rays, rays->n_steps, A.M);   // what the forward left in `saved`
     A.g_depth = g_depth; A.g_image = g_image; A.g_wsum = g_wsum; A.g_weights = g_weights;
@@ -1370,19 +1448,20 @@ extern "C" int l4d_render_backward_ex(const L4DConfig* cfg, const void* staged, 
     }
     {
       int grid;
-      rc = grid_for(k_bwd_scatter<L4D_NT, L4D_SCATTER_MIN_CTAS>, L4D_NT, 0, tiles, grid);
+      auto scatter = mf ? k_bwd_scatter<L4D_NT, L4D_SCATTER_MIN_CTAS, true> : k_bwd_scatter<L4D_NT, L4D_SCATTER_MIN_CTAS, false>;
+      rc = grid_for(scatter, L4D_NT, 0, tiles, grid);
       if (rc != L4D_OK) return rc;
-      ++g_launches; k_bwd_scatter<L4D_NT, L4D_SCATTER_MIN_CTAS><<<grid, L4D_NT, 0, st>>>(A);
+      ++g_launches; scatter<<<grid, L4D_NT, 0, st>>>(A);
       prof_mark(st, "k_bwd_scatter");
-      {       // gradient rows -> the two live time rows of every time plane
+      for (uint32_t f = 0; f < frames->n_frames; ++f) {       // gradient rows -> the two live time rows of every time plane
         TimeRowArgs T;
-        fill_time_rows(T, cfg, frame);
+        fill_time_rows(T, cfg, &frames->frames[f]);
         uint32_t rmax = 0;
         for (uint32_t s2 = 0; s2 < cfg->n_plane_scales; ++s2) {
           rmax = cfg->plane_res[s2] > rmax ? cfg->plane_res[s2] : rmax;
           for (int t = 0; t < 3; ++t) {
             T.plane[s2][t] = A.G.planes_cl[s2][t == 0 ? 2 : (t == 1 ? 4 : 5)];
-            for (int q = 0; q < 3; ++q) T.row[s2][t][q] = A.G.pl_rows[s2][t][q];
+            for (int q = 0; q < 3; ++q) T.row[s2][t][q] = A.G.pl_rows[s2][t][q] + f * A.comb_fstride;
           }
         }
         ++g_launches; k_fold_planes<<<dim3((unsigned)nblk((size_t)rmax * 8), 3 * cfg->n_plane_scales), 256, 0, st>>>(T);
@@ -1391,20 +1470,25 @@ extern "C" int l4d_render_backward_ex(const L4DConfig* cfg, const void* staged, 
       if (rc != L4D_OK) return rc;
       ++g_launches; k_bwd_scatter_static<L4D_NT><<<grid, L4D_NT, 0, st>>>(A);
       prof_mark(st, "k_bwd_scatter_static");
-      for (int p = 0; p < 3; ++p) {
-        const size_t n = cfg->hash_dynamic[p].offset[cfg->hash_dynamic[p].n_levels];
-        const bool single = frame->cur.single != 0;
-        const float* tb = frame->cur.basis;
-        ++g_launches; k_fold_dynamic<<<nblk(n), 256, 0, st>>>(A.G.hd_comb[p],
-                                               reinterpret_cast<float4*>(A.G.hd[p][frame->cur.slice_lo]),
-                                               single ? nullptr : reinterpret_cast<float4*>(A.G.hd[p][frame->cur.slice_hi]), n,
-                                               single ? 1.0f : frame->cur.w_lo, frame->cur.w_hi, tb[0], tb[1], tb[2], tb[3]);
+      for (uint32_t f = 0; f < frames->n_frames; ++f) {
+        const L4DFrame* frame = &frames->frames[f];
+        for (int p = 0; p < 3; ++p) {
+          const size_t n = cfg->hash_dynamic[p].offset[cfg->hash_dynamic[p].n_levels];
+          const bool single = frame->cur.single != 0;
+          const float* tb = frame->cur.basis;
+          ++g_launches; k_fold_dynamic<<<nblk(n), 256, 0, st>>>(A.G.hd_comb[p] + f * A.comb_fstride,
+                                                 reinterpret_cast<float4*>(A.G.hd[p][frame->cur.slice_lo]),
+                                                 single ? nullptr : reinterpret_cast<float4*>(A.G.hd[p][frame->cur.slice_hi]), n,
+                                                 single ? 1.0f : frame->cur.w_lo, frame->cur.w_hi, tb[0], tb[1], tb[2], tb[3]);
+        }
       }
       prof_mark(st, "k_fold_dynamic");
       // hash_static and hash_dynamic gradients are final from here on (the flow backward below only touches the flow net)
       if (ev_hash_done) L4D_CUDA(cudaEventRecord((cudaEvent_t)ev_hash_done, st));
     }
-    if (frame->has_fwd || frame->has_bwd) {     // with no neighbour frame nothing reaches the flow field
+    bool any_neighbour = false;
+    for (uint32_t f = 0; f < frames->n_frames; ++f) any_neighbour |= frames->frames[f].has_fwd || frames->frames[f].has_bwd;
+    if (any_neighbour) {     // with no neighbour frame nothing reaches the flow field (samples of such frames give dL/dflow = 0)
       if (cfg->mlp_fp16) {
         const size_t smem = tc_dyn_smem(flow_tc_smem().total);
         int grid;
@@ -1412,12 +1496,18 @@ extern "C" int l4d_render_backward_ex(const L4DConfig* cfg, const void* staged, 
         if (rc != L4D_OK) return rc;
         ++g_launches; k_bwd_flow_tc<<<grid, 128, smem, st>>>(A);
         prof_mark(st, "k_bwd_flow_tc");
-        rc = grid_for(k_bwd_flowgrid<L4D_NT>, L4D_NT, 0, tiles, grid);
+        auto flowgrid = mf ? k_bwd_flowgrid<L4D_NT, true> : k_bwd_flowgrid<L4D_NT, false>;
+        rc = grid_for(flowgrid, L4D_NT, 0, tiles, grid);
         if (rc != L4D_OK) return rc;
-        ++g_launches; k_bwd_flowgrid<L4D_NT><<<grid, L4D_NT, 0, st>>>(A);
+        ++g_launches; flowgrid<<<grid, L4D_NT, 0, st>>>(A);
         const size_t n = cfg->flow.offset[cfg->flow.n_levels];
-        const float* fb = frame->flow_basis;
-        ++g_launches; k_fold_flow<<<nblk(n), 256, 0, st>>>(reinterpret_cast<float2*>(A.G.hf_comb), reinterpret_cast<float4*>(A.G.hf), n, fb[0], fb[1], fb[2], fb[3]);
+        for (uint32_t f = 0; f < frames->n_frames; ++f) {
+          const L4DFrame* frame = &frames->frames[f];
+          if (!frame->has_fwd && !frame->has_bwd) continue;       // its accumulator received zeros only
+          const float* fb = frame->flow_basis;
+          ++g_launches; k_fold_flow<<<nblk(n), 256, 0, st>>>(reinterpret_cast<float2*>(A.G.hf_comb + f * A.comb_fstride),
+                                                             reinterpret_cast<float4*>(A.G.hf), n, fb[0], fb[1], fb[2], fb[3]);
+        }
         prof_mark(st, "k_bwd_flowgrid");
       } else {
         const size_t smem = (64 * L4D_NT + 2 * L4D_NT * L4D_TILE_LD) * sizeof(float);
@@ -1435,7 +1525,7 @@ extern "C" int l4d_render_backward_ex(const L4DConfig* cfg, const void* staged, 
   memset(&A, 0, sizeof(A));
   build_model(cfg, staged, A.M);
   build_grads(cfg, grads, grad_work, A.G);
-  A.F = *frame;
+  A.FT = *frames;
   A.rays_o = rays->rays_o; A.rays_d = rays->rays_d;
   A.n_rays = rays->n_rays; A.S = rays->n_steps; A.perturb = rays->perturb;
   A.seed = rays->seed; A.ray_offset = rays->ray_offset;

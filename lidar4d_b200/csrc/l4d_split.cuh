@@ -19,7 +19,9 @@
 
 struct SplitArgs {
   DevModel M;
-  L4DFrame F;
+  L4DFrameTable FT;     // frame of every ray (l4d_frame_of); the per-frame tables below sit con_fstride / comb_fstride apart
+  size_t con_fstride;   // floats between two frames' contracted tables (DevModel::hd_con, pl_con)
+  size_t comb_fstride;  // floats between two frames' accumulators (DevGrads::hd_comb, hf_comb, pl_rows)
   DevGrads G;
   const float* rays_o;
   const float* rays_d;
@@ -80,7 +82,8 @@ __device__ __forceinline__ void l4d_static_sweep(const SplitArgs& A, const RaySa
 #ifndef L4D_GATHER_MIN_CTAS
 #define L4D_GATHER_MIN_CTAS 6
 #endif
-template <int NT, bool FLOW_GIVEN, bool TILE>
+// MF: several frames in the launch (l4d_frame_of)
+template <int NT, bool FLOW_GIVEN, bool TILE, bool MF>
 __global__ void __launch_bounds__(NT, FLOW_GIVEN ? L4D_GATHER_MIN_CTAS : 4) k_fwd_gather(const __grid_constant__ SplitArgs A) {
   extern __shared__ __align__(16) float smem[];
   float* xb = smem + threadIdx.x;          // exchange column for the flow MLP, stride NT
@@ -100,6 +103,8 @@ __global__ void __launch_bounds__(NT, FLOW_GIVEN ? L4D_GATHER_MIN_CTAS : 4) k_fw
       continue;
     }
     const size_t p = (size_t)ray * A.S + j;
+    const uint32_t fi = l4d_frame_of<MF>(A.FT, ray);
+    const L4DFrame& F = A.FT.frames[fi];
     const float zj = l4d_z(rs, A.ray_offset + ray, j);
     const float x = l4d_x01(__ldg(A.rays_o + 3 * ray), __ldg(A.rays_d + 3 * ray), zj, M.bound);
     const float y = l4d_x01(__ldg(A.rays_o + 3 * ray + 1), __ldg(A.rays_d + 3 * ray + 1), zj, M.bound);
@@ -110,7 +115,7 @@ __global__ void __launch_bounds__(NT, FLOW_GIVEN ? L4D_GATHER_MIN_CTAS : 4) k_fw
       for (int k = 0; k < 6; ++k) flow[k] = __ldg(A.sv.flow + (size_t)k * P + p);
       flow[6] = flow[7] = 0.f;
     } else {
-      l4d_flow_inputs(M, A.F.flow_basis, x, y, z, xb, NT, A.sv.flow_in + p, P);
+      l4d_flow_inputs(M, F.flow_basis, x, y, z, xb, NT, A.sv.flow_in + p, P);
       uint32_t a, b, c, d;
       l4d_flow_mlp(M, xb, NT, flow, a, b, c, d);
 #pragma unroll
@@ -120,7 +125,7 @@ __global__ void __launch_bounds__(NT, FLOW_GIVEN ? L4D_GATHER_MIN_CTAS : 4) k_fw
     sink.feat = TILE ? nullptr : A.sv.feat; sink.P = P; sink.p = p; sink.dense = nullptr;
     sink.tile = tile; sink.tile_lo = lo_off;
     float dummy[L4D_H];
-    l4d_gather_features<false, false>(M, A.F, x, y, z, flow, xb, NT, sink, dummy);      // static hash: below
+    l4d_gather_features<false, false>(M, F, x, y, z, flow, xb, NT, sink, dummy, fi * A.con_fstride);   // static hash: below
     if (TILE) {                             // tcnn's ones-padding inside the last stored chunk
       for (uint32_t k = M.sigma_in_dim; k < A.sv.x_chunks * 8u; ++k) {
         unsigned char* q = tile + (size_t)(k >> 3) * 2048 + (size_t)(k & 7u) * 2;
@@ -359,8 +364,9 @@ struct DfeatFromTile {
   }
 };
 
-// the time planes come from the forward's contracted rows (DevModel::pl_con) and reduce into DevGrads::pl_rows
-template <int NT, int MIN_CTAS>
+// the time planes come from the forward's contracted rows (DevModel::pl_con) and reduce into DevGrads::pl_rows, both those of
+// the sample's frame
+template <int NT, int MIN_CTAS, bool MF>
 __global__ void __launch_bounds__(NT, MIN_CTAS) k_bwd_scatter(const __grid_constant__ SplitArgs A) {
   const DevModel& M = A.M;
   const size_t P = A.sv.P;
@@ -380,7 +386,9 @@ __global__ void __launch_bounds__(NT, MIN_CTAS) k_bwd_scatter(const __grid_const
 #pragma unroll
     for (int k = 0; k < 6; ++k) flow[k] = A.sv.flow[(size_t)k * P + p];
     DfeatFromTile df{A.sv.dfeat + l4d_dfeat_off(A.sv, ray, j), active};
-    l4d_bw_scatter_t<true, DfeatFromTile, false, true>(M, A.F, A.G, x, y, z, flow, df, dflow, active, (int)ray);
+    const uint32_t fi = l4d_frame_of<MF>(A.FT, ray);
+    l4d_bw_scatter_t<true, DfeatFromTile, false, true>(M, A.FT.frames[fi], A.G, x, y, z, flow, df, dflow, active, (int)ray, fi,
+                                                       fi * A.con_fstride, fi * A.comb_fstride);
     if (active) {
 #pragma unroll
       for (int k = 0; k < 6; ++k) A.sv.dflow[(size_t)k * P + p] = dflow[k];
@@ -410,9 +418,10 @@ __global__ void __launch_bounds__(NT) k_bwd_flow(const __grid_constant__ SplitAr
     s.masked = false;
     s.x = s.y = s.z = 0.f;
     const size_t p = s.active ? pp : 0;
+    const uint32_t ray = (uint32_t)(p / A.S), j = (uint32_t)(p % A.S);
+    const L4DFrame& F = A.FT.frames[l4d_frame_of(A.FT, ray)];
     float g[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     if (s.active) {
-      const uint32_t ray = (uint32_t)(p / A.S), j = (uint32_t)(p % A.S);
       const float zj = l4d_z(rs, A.ray_offset + ray, j);
       s.x = l4d_x01(__ldg(A.rays_o + 3 * ray), __ldg(A.rays_d + 3 * ray), zj, M.bound);
       s.y = l4d_x01(__ldg(A.rays_o + 3 * ray + 1), __ldg(A.rays_d + 3 * ray + 1), zj, M.bound);
@@ -429,7 +438,7 @@ __global__ void __launch_bounds__(NT) k_bwd_flow(const __grid_constant__ SplitAr
     __syncthreads();
     tile_outer_accum<NT>(TA, TB, 64, A.G.flo_w1t);
     __syncthreads();
-    l4d_bw_flow_c(M, A.F, A.G, s, A.sv.flow_in + p, P, xb, NT, ta_row, tb_row);
+    l4d_bw_flow_c(M, F, A.G, s, A.sv.flow_in + p, P, xb, NT, ta_row, tb_row);
     __syncthreads();
     tile_outer_accum<NT>(TA, TB, 16, A.G.flo_w0t);
   }
@@ -445,17 +454,18 @@ __global__ void __launch_bounds__(NT) k_bwd_flow(const __grid_constant__ SplitAr
 #ifndef L4D_FLOWGRID_MIN_CTAS
 #define L4D_FLOWGRID_MIN_CTAS 4
 #endif
-template <int NT>
+template <int NT, bool MF>
 __global__ void __launch_bounds__(NT, L4D_FLOWGRID_MIN_CTAS) k_bwd_flowgrid(const __grid_constant__ SplitArgs A) {
   const DevModel& M = A.M;
   const size_t P = A.sv.P;
   const RaySampling rs = l4d_make_sampling(M.near_lidar, M.far_lidar, A.S, A.perturb, A.seed);
-  const float* b = A.F.flow_basis;
   for (size_t base = (size_t)blockIdx.x * NT; base < P; base += (size_t)gridDim.x * NT) {
     const size_t pp = base + threadIdx.x;
     const bool active = pp < P;
     const size_t p = active ? pp : P - 1;
     const uint32_t ray = (uint32_t)(p / A.S), j = (uint32_t)(p % A.S);
+    const uint32_t fi = l4d_frame_of<MF>(A.FT, ray);
+    const float* b = A.FT.frames[fi].flow_basis;
     const float zj = l4d_z(rs, A.ray_offset + ray, j);
     const float x = l4d_x01(__ldg(A.rays_o + 3 * ray), __ldg(A.rays_d + 3 * ray), zj, M.bound);
     const float y = l4d_x01(__ldg(A.rays_o + 3 * ray + 1), __ldg(A.rays_d + 3 * ray + 1), zj, M.bound);
@@ -467,12 +477,13 @@ __global__ void __launch_bounds__(NT, L4D_FLOWGRID_MIN_CTAS) k_bwd_flowgrid(cons
       uint32_t idx[8]; float w[8];
       l4d_corners3(M.gf, l, x, y, z, idx, w);
       float* gb = A.G.hf + (size_t)M.gf.offset[l] * 8;
-      float* gc = A.G.hf_comb ? A.G.hf_comb + (size_t)M.gf.offset[l] * 2 : nullptr;    // basis applied by k_fold_flow
+      float* gc = A.G.hf_comb ? A.G.hf_comb + fi * A.comb_fstride + (size_t)M.gf.offset[l] * 2 : nullptr;   // basis: k_fold_flow
       if (M.gf.res[l] <= 400u) {            // warp-uniform: aggregate runs of equal cells
         uint32_t cx, cy, cz; float fx, fy, fz;
         const float sc = M.gf.scale[l];
         l4d_pos_fract(sc, x, cx, fx); l4d_pos_fract(sc, y, cy, fy); l4d_pos_fract(sc, z, cz, fz);
-        const WarpRuns r = l4d_warp_runs((int)(cx + M.gf.res[l] * (cy + M.gf.res[l] * cz)));
+        // runs never join two frames: their sums go to different accumulators (cell indices stay below 400^3 < 2^26)
+        const WarpRuns r = l4d_warp_runs((int)(cx + M.gf.res[l] * (cy + M.gf.res[l] * cz) + (fi << 26)));
         float s0[8], s1[8];
 #pragma unroll
         for (int c = 0; c < 8; ++c) { s0[c] = w[c] * d0; s1[c] = w[c] * d1; }

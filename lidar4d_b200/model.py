@@ -375,15 +375,17 @@ class _Engine:
             _capi.fill_pointer_table(self._gtab, self.cfg, lambda n: base + 4 * self.offsets[n][0])
         return self._gtab
 
-    def work(self):
+    def work(self, n_frames: int = 1):
         """Persistent zero-initialised gradient work buffer (plane / MLP grads in working layout, slice-independent
-        hash accumulators) of the CURRENT stream: every kernel that consumes a region clears it again, so launches
-        that overlap on different streams need their own (a fold kernel of one must not clear what the scatter of the
-        other is still adding)."""
+        hash accumulators, once per frame of a multi-frame launch) of the CURRENT stream: every kernel that consumes a
+        region clears it again, so launches that overlap on different streams need their own (a fold kernel of one must
+        not clear what the scatter of the other is still adding).  Grows on demand to the size of n_frames frames."""
         key = (self.device(), self.stream())
         w = self._works.get(key)
-        if w is None:
-            n = self._lib().l4d_grad_work_bytes(C.byref(self.ccfg))
+        n = self._lib().l4d_grad_work_bytes_frames(C.byref(self.ccfg), n_frames)
+        if n == 0:
+            raise RuntimeError("l4d_grad_work_bytes_frames: " + self._lib().l4d_last_error().decode())
+        if w is None or w.numel() < n:
             w = self._works[key] = torch.zeros(n, dtype=torch.uint8, device=self.device())
         return w
 
@@ -392,9 +394,9 @@ class _Engine:
         for w in self._works.values():
             w.zero_()
 
-    def infer_workspace(self, n_rays: int, S: int):
+    def infer_workspace(self, n_rays: int, S: int, n_frames: int = 1):
         """Persistent exchange workspace of no-grad renders through the split pipeline (grown on demand)."""
-        n = self._lib().l4d_saved_bytes(C.byref(self.ccfg), n_rays, S)
+        n = self._lib().l4d_saved_bytes_frames(C.byref(self.ccfg), n_rays, S, n_frames)
         ws = getattr(self, "_infer_ws", None)
         if ws is None or ws.device != self.device() or ws.numel() < n:
             self._infer_ws = ws = torch.empty(n, dtype=torch.uint8, device=self.device())
@@ -492,6 +494,35 @@ class _Engine:
             time = float(time.reshape(-1)[0])          # same host sync as lidar4d.py:143
         return _capi.make_frame_struct(make_frame(time, self.cfg.num_frames, self.cfg.time_resolution))
 
+    def render_frames(self, time, rays_shape):
+        """The frames of a render call as [(first row, rows, L4DFrame or L4DFrameTable)]: one L4DFrame for a single time
+        (a float or a one-element tensor) or for B equal row times; otherwise one frame per row of rays [B, N, 3], in
+        tables of at most MAX_FRAMES rows.  One device->host read of the times, as for one frame."""
+        if not torch.is_tensor(time) or time.numel() == 1:
+            return [(0, None, self.frame(time))]
+        B = rays_shape[0] if len(rays_shape) == 3 else None
+        if B is None or time.numel() != B or tuple(time.shape) not in ((B,), (B, 1)):
+            raise ValueError(f"time must be one value or one per row of rays [B, N, 3] (shape [B] or [B, 1]); got time "
+                             f"{tuple(time.shape)} for rays {tuple(rays_shape)}")
+        times = time.detach().reshape(-1).tolist()
+        if all(t == times[0] for t in times):
+            return [(0, None, _capi.make_frame_struct(make_frame(times[0], self.cfg.num_frames, self.cfg.time_resolution)))]
+        return [(b0, len(rows), _capi.make_frame_table(rows, rays_shape[1]))
+                for b0, rows in row_frame_groups(self.cfg, times)]
+
+
+def row_frame_groups(cfg, times):
+    """[(first row, [L4DFrame of each row])] in groups of at most MAX_FRAMES rows: make_frame of every row's time."""
+    frames = [_capi.make_frame_struct(make_frame(t, cfg.num_frames, cfg.time_resolution)) for t in times]
+    return [(b0, frames[b0:b0 + _capi.MAX_FRAMES]) for b0 in range(0, len(frames), _capi.MAX_FRAMES)]
+
+
+def _sub_table(tab: _capi.L4DFrameTable, h: int, n: int) -> _capi.L4DFrameTable:
+    """The frames of rays [h, h + n) of a launch over `tab`."""
+    rpf, ph = tab.rays_per_frame, tab.first_ray_phase + h
+    first, last = ph // rpf, (ph + n - 1) // rpf
+    return _capi.make_frame_table([tab.frames[i] for i in range(first, last + 1)], rpf, ph % rpf)
+
 
 class _RenderFn(torch.autograd.Function):
     """Fused render forward / backward.  Parameters are passed as inputs so that autograd schedules the backward;
@@ -501,7 +532,10 @@ class _RenderFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, eng: _Engine, rays_o, rays_d, frame, S, perturb, seed, ray_offset, want_weights, train, *params):
+        """frame: one L4DFrame for every ray, or an L4DFrameTable (several frames in one launch)."""
         lib = eng._lib()
+        multi = isinstance(frame, _capi.L4DFrameTable)
+        n_frames = frame.n_frames if multi else 1
         N = rays_o.shape[0]
         dev = rays_o.device
         depth = torch.empty(N, device=dev)
@@ -518,13 +552,13 @@ class _RenderFn(torch.autograd.Function):
         saved, nsaved = None, 0
         chunk = N
         if train:
-            nsaved = lib.l4d_saved_bytes(C.byref(eng.ccfg), N, S)
+            nsaved = lib.l4d_saved_bytes_frames(C.byref(eng.ccfg), N, S, n_frames)
             saved = torch.empty(nsaved, dtype=torch.uint8, device=dev)
         elif not fused:
             # inference through the split pipeline: the kernels exchange feature tiles through a workspace; walk the rays
             # in chunks over ONE persistent workspace (config 4: 131,072 rays per frame would otherwise need 160 GB)
             chunk = min(N, int(eng.owner.infer_ray_chunk))
-            saved, nsaved = eng.infer_workspace(chunk, S)
+            saved, nsaved = eng.infer_workspace(chunk, S, n_frames)
         ev = eng._events("fwd")
         with torch.cuda.device(dev):
             if ev: ev[0].record()
@@ -532,8 +566,10 @@ class _RenderFn(torch.autograd.Function):
                 n = min(chunk, N - h)
                 rays.rays_o, rays.rays_d, rays.n_rays = rays_o.data_ptr() + 12 * h, rays_d.data_ptr() + 12 * h, n
                 rays.ray_offset = int(ray_offset) + h
-                rc = lib.l4d_render_forward(
-                    C.byref(eng.ccfg), eng.staged.data_ptr(), C.byref(frame), C.byref(rays),
+                fwd = lib.l4d_render_forward_frames if multi else lib.l4d_render_forward
+                fr = _sub_table(frame, h, n) if multi and n < N else frame
+                rc = fwd(
+                    C.byref(eng.ccfg), eng.staged.data_ptr(), C.byref(fr), C.byref(rays),
                     depth.data_ptr() + 4 * h, image.data_ptr() + 8 * h, wsum.data_ptr() + 4 * h,
                     weights.data_ptr() + 4 * h * S if want_weights else None, zvals.data_ptr() + 4 * h * S if want_weights else None,
                     saved.data_ptr() if saved is not None else None, nsaved, eng.stream())
@@ -566,7 +602,8 @@ class _RenderFn(torch.autograd.Function):
         g_weights = None if g_weights is None else g_weights.contiguous().float()
         arena = eng.owner.grad_mode == "arena"
         tab, views = (eng.attach_grads(), None) if arena else _scratch_grads(eng)
-        work = eng.work()
+        multi = isinstance(ctx.frame, _capi.L4DFrameTable)
+        work = eng.work(ctx.frame.n_frames if multi else 1)
         rays = _capi.L4DRays()
         rays.rays_o, rays.rays_d = ctx.rays_o.data_ptr(), ctx.rays_d.data_ptr()
         rays.n_rays, rays.n_steps, rays.perturb, rays.seed, rays.ray_offset = N, S, perturb, seed, ray_offset
@@ -575,7 +612,8 @@ class _RenderFn(torch.autograd.Function):
         with torch.cuda.device(dev):
             if ev: ev[0].record()
             hook = eng.hash_grads_hook if arena else None      # (event, callback) armed by RayShardedDP for the step's last backward
-            rc = lib.l4d_render_backward_ex(
+            bwd = lib.l4d_render_backward_frames if multi else lib.l4d_render_backward_ex
+            rc = bwd(
                 C.byref(eng.ccfg), eng.staged.data_ptr(), C.byref(ctx.frame), C.byref(rays),
                 ctx.saved.data_ptr(), ctx.nsaved, g_depth.data_ptr(), g_image.data_ptr(),
                 g_wsum.data_ptr() if g_wsum is not None else None,
@@ -1029,7 +1067,7 @@ class LiDAR4D(LiDAR_Renderer):
         rd = rays_d.detach().contiguous().view(-1, 3).float()
         eng._require_cuda(ro, rd)
         eng.ensure_staged()
-        frame = eng.frame(time)
+        groups = eng.render_frames(time, tuple(rays_o.shape))
         params = self._params_list()
         train = torch.is_grad_enabled() and any(p.requires_grad for p in params)
         seed = 0
@@ -1037,7 +1075,16 @@ class LiDAR4D(LiDAR_Renderer):
             seed = self.jitter_seed + self._jitter_calls
             self._jitter_calls += 1
         want_w = bool(self.materialize_weights)
-        out = _RenderFn.apply(eng, ro, rd, frame, int(num_steps), bool(perturb), seed, int(ray_offset), want_w, train, *params)
+        if len(groups) == 1 and groups[0][1] is None:
+            out = _RenderFn.apply(eng, ro, rd, groups[0][2], int(num_steps), bool(perturb), seed, int(ray_offset), want_w,
+                                  train, *params)
+        else:
+            # one launch per table of rows; ray (b, j) keeps the jitter index ray_offset + b * N + j of the flattened launch
+            N = rays_o.shape[1]
+            outs = [_RenderFn.apply(eng, ro[b0 * N:(b0 + k) * N], rd[b0 * N:(b0 + k) * N], tab, int(num_steps),
+                                    bool(perturb), seed, int(ray_offset) + b0 * N, want_w, train, *params)
+                    for b0, k, tab in groups]
+            out = outs[0] if len(outs) == 1 else tuple(torch.cat(parts) for parts in zip(*outs))
         res = {"depth_lidar": out[0].view(*prefix), "image_lidar": out[1].view(*prefix, self.out_lidar_dim),
                "weights_sum_lidar": out[2]}
         if want_w:
