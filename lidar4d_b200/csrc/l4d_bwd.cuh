@@ -654,7 +654,7 @@ L4D_HD void l4d_bw_scatter_t(const DevModel& M, const L4DFrame& F, const DevGrad
   }
 
   // static hash: dL/dtable[entry] += w_corner * dfeat[0..4)   (the split pipeline does this level-major in
-  // k_bwd_scatter_static so that only one level's 8 MB of gradients is live in L2 at a time)
+  // k_bwd_encoders so that only one level's 8 MB of gradients is live in L2 at a time)
 #pragma unroll 1
   for (int l = 0; STATIC_HASH && active && l < L; ++l) {
     uint32_t idx[8]; float w[8];

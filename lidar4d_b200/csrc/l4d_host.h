@@ -23,6 +23,7 @@ struct GradWorkLayout {
   size_t sig_w1t, sig_w2;
   size_t att_w1t[2], att_w2t[2], att_w3[2];
   size_t flo_w0t, flo_w1t, flo_w2;
+  size_t scatter_tickets;  // 3 x uint32: k_bwd_encoders' work-ticket counters
   size_t hd_comb[3], hf_comb;
   size_t pl_rows;          // [query][scale][plane 2|4|5][R][8]
   size_t comb_frame;       // bytes of one frame's hd_comb .. pl_rows block; frame f's block is at + f * comb_frame
@@ -116,6 +117,7 @@ static inline GradWorkLayout grad_work_layout(const L4DConfig* c, uint32_t n_fra
   L.flo_w0t = take(16 * 64 * f);
   L.flo_w1t = take(64 * 64 * f);
   L.flo_w2 = take(8 * 64 * f);
+  L.scatter_tickets = take(3 * sizeof(uint32_t));
   for (int p = 0; p < 3; ++p) L.hd_comb[p] = take((size_t)c->hash_dynamic[p].offset[c->hash_dynamic[p].n_levels] * f);
   L.hf_comb = take((size_t)c->flow.offset[c->flow.n_levels] * 2 * f);
   L.pl_rows = take(time_rows_floats(c) * f);

@@ -1448,11 +1448,14 @@ extern "C" int l4d_render_backward_frames(const L4DConfig* cfg, const void* stag
     }
     {
       int grid;
-      auto scatter = mf ? k_bwd_scatter<L4D_NT, L4D_SCATTER_MIN_CTAS, true> : k_bwd_scatter<L4D_NT, L4D_SCATTER_MIN_CTAS, false>;
-      rc = grid_for(scatter, L4D_NT, 0, tiles, grid);
+      auto scatter = mf ? k_bwd_encoders<L4D_NT, true> : k_bwd_encoders<L4D_NT, false>;
+      rc = grid_for(scatter, L4D_NT, 0, tiles * (1u + cfg->hash_static.n_levels), grid);
       if (rc != L4D_OK) return rc;
-      ++g_launches; scatter<<<grid, L4D_NT, 0, st>>>(A);
-      prof_mark(st, "k_bwd_scatter");
+      // the static-hash CTAs: L4D_SCATTER_STATIC_PER_SM of every L4D_SCATTER_MIN_CTAS, the first ones dispatched
+      const uint32_t n_static = ((uint32_t)grid * L4D_SCATTER_STATIC_PER_SM + L4D_SCATTER_MIN_CTAS - 1) / L4D_SCATTER_MIN_CTAS;
+      A.scatter_tickets = reinterpret_cast<uint32_t*>(static_cast<char*>(grad_work) + grad_work_layout(cfg).scatter_tickets);
+      ++g_launches; scatter<<<grid, L4D_NT, 0, st>>>(A, n_static);
+      prof_mark(st, "k_bwd_encoders");
       for (uint32_t f = 0; f < frames->n_frames; ++f) {       // gradient rows -> the two live time rows of every time plane
         TimeRowArgs T;
         fill_time_rows(T, cfg, &frames->frames[f]);
@@ -1466,10 +1469,7 @@ extern "C" int l4d_render_backward_frames(const L4DConfig* cfg, const void* stag
         }
         ++g_launches; k_fold_planes<<<dim3((unsigned)nblk((size_t)rmax * 8), 3 * cfg->n_plane_scales), 256, 0, st>>>(T);
       }
-      rc = grid_for(k_bwd_scatter_static<L4D_NT>, L4D_NT, 0, tiles, grid);
-      if (rc != L4D_OK) return rc;
-      ++g_launches; k_bwd_scatter_static<L4D_NT><<<grid, L4D_NT, 0, st>>>(A);
-      prof_mark(st, "k_bwd_scatter_static");
+      prof_mark(st, "k_fold_planes");
       for (uint32_t f = 0; f < frames->n_frames; ++f) {
         const L4DFrame* frame = &frames->frames[f];
         for (int p = 0; p < 3; ++p) {

@@ -10,8 +10,8 @@
 // which the otherwise idle HBM absorbs.  Same per-sample functions (l4d_core.cuh / l4d_bwd.cuh), same numerics.
 //
 //   forward :  [k_fwd_flow_tc ->] k_fwd_gather -> k_fwd_dense{,_tc}
-//   backward:  k_bwd_dense{,_tc} -> k_bwd_scatter + k_bwd_scatter_static -> k_fold_dynamic
-//              -> k_bwd_flow  |  k_bwd_flow_tc -> k_bwd_flowgrid -> k_fold_flow
+//   backward:  k_bwd_dense{,_tc} -> k_bwd_encoders (encoder and static-hash scatter side by side) -> k_fold_planes
+//              -> k_fold_dynamic -> k_bwd_flow  |  k_bwd_flow_tc -> k_bwd_flowgrid -> k_fold_flow
 // (the *_tc kernels live in l4d_dense_tc.cuh; DESIGN.md 4.2 has the measured time and limiter of each)
 #pragma once
 #include "l4d_bwd.cuh"
@@ -30,9 +30,10 @@ struct SplitArgs {
   float *depth, *image, *wsum, *weights, *zvals;
   const float *g_depth, *g_image, *g_wsum, *g_weights;
   SavedView sv;
+  uint32_t* scatter_tickets;   // k_bwd_encoders' work-ticket counters (grad_work, zero between launches)
 };
 
-// static-hash rows of k_fwd_gather, LEVEL-MAJOR (the forward twin of k_bwd_scatter_static).  The fp16 static table is 4 MB per
+// static-hash rows of k_fwd_gather, LEVEL-MAJOR (the forward twin of the static-hash work of k_bwd_encoders).  The fp16 static table is 4 MB per
 // hashed level (64 MB at L = 16, more than the H100's 50 MB L2): gathered sample-major, all levels are live at once.  Here every
 // CTA sweeps its samples once per level PAIR, so the chip reads 8 MB of the table at a time.  row_hash_s is a multiple of 16,
 // so a pair fills one 16-byte chunk of an operand-tile row and a warp stores 512 contiguous bytes per half.  Same per-sample
@@ -344,13 +345,14 @@ __global__ void __launch_bounds__(NT) k_bwd_dense(const __grid_constant__ SplitA
 }
 
 // -------------------------------------------------------------------------------------------
-// backward 2/3: scatter dL/dfeature through the encoders (vector REDs), thread == sample.
+// backward 2/3, encoder work: scatter dL/dfeature through the planes, time rows and dynamic hash (vector REDs),
+// thread == sample; one block of NT consecutive samples per call (k_bwd_encoders below runs it).
 // -------------------------------------------------------------------------------------------
-// H100 80GB HBM3 at a 400 W power limit, L = 16, ms per launch of 16,384 rays: 3 CTAs/SM 27.1 (168 registers, 16 B of spill
-// stores), 4: 26.3-26.9 (128, 36 B), 5: 29.4 (96, 224 B) -> 4 (short runs, before the dynamic hash's vertex runs).  With the
-// contracted time rows (the benchmark's kernel) at 4: 36.1-36.2 ms (128 registers, 36 B of spill stores) before the vertex
-// runs, 31.8-31.9 (128, 48 B) with them; 18.7 with the dynamic hash left out (a scratch build), so the dynamic hash went from
-// 17.5 to about 13.2 ms of it.
+// As a kernel of its own (k_bwd_scatter) on an H100 80GB HBM3 at a 400 W power limit, L = 16, ms per launch of 16,384 rays:
+// 3 CTAs/SM 27.1 (168 registers, 16 B of spill stores), 4: 26.3-26.9 (128, 36 B), 5: 29.4 (96, 224 B) -> 4 (short runs, before
+// the dynamic hash's vertex runs).  With the contracted time rows (the benchmark's kernel) at 4: 36.1-36.2 ms (128 registers,
+// 36 B of spill stores) before the vertex runs, 31.8-31.9 (128, 48 B) with them; 18.7 with the dynamic hash left out (a scratch
+// build), so the dynamic hash went from 17.5 to about 13.2 ms of it.
 #ifndef L4D_SCATTER_MIN_CTAS
 #define L4D_SCATTER_MIN_CTAS 4
 #endif
@@ -366,33 +368,31 @@ struct DfeatFromTile {
 
 // the time planes come from the forward's contracted rows (DevModel::pl_con) and reduce into DevGrads::pl_rows, both those of
 // the sample's frame
-template <int NT, int MIN_CTAS, bool MF>
-__global__ void __launch_bounds__(NT, MIN_CTAS) k_bwd_scatter(const __grid_constant__ SplitArgs A) {
+template <int NT, bool MF>
+__device__ __forceinline__ void l4d_encoder_scatter_block(const SplitArgs& A, size_t base) {
   const DevModel& M = A.M;
   const size_t P = A.sv.P;
   const RaySampling rs = l4d_make_sampling(M.near_lidar, M.far_lidar, A.S, A.perturb, A.seed);
-  for (size_t base = (size_t)blockIdx.x * NT; base < P; base += (size_t)gridDim.x * NT) {
-    // whole warps stay together (plane gradients are aggregated across lanes); lanes past the end
-    // shadow the last sample with zero gradient
-    const size_t pp = base + threadIdx.x;
-    const bool active = pp < P;
-    const size_t p = active ? pp : P - 1;
-    const uint32_t ray = (uint32_t)(p / A.S), j = (uint32_t)(p % A.S);
-    const float zj = l4d_z(rs, A.ray_offset + ray, j);
-    const float x = l4d_x01(__ldg(A.rays_o + 3 * ray), __ldg(A.rays_d + 3 * ray), zj, M.bound);
-    const float y = l4d_x01(__ldg(A.rays_o + 3 * ray + 1), __ldg(A.rays_d + 3 * ray + 1), zj, M.bound);
-    const float z = l4d_x01(__ldg(A.rays_o + 3 * ray + 2), __ldg(A.rays_d + 3 * ray + 2), zj, M.bound);
-    float flow[6], dflow[6];
+  // whole warps stay together (plane gradients are aggregated across lanes); lanes past the end
+  // shadow the last sample with zero gradient
+  const size_t pp = base + threadIdx.x;
+  const bool active = pp < P;
+  const size_t p = active ? pp : P - 1;
+  const uint32_t ray = (uint32_t)(p / A.S), j = (uint32_t)(p % A.S);
+  const float zj = l4d_z(rs, A.ray_offset + ray, j);
+  const float x = l4d_x01(__ldg(A.rays_o + 3 * ray), __ldg(A.rays_d + 3 * ray), zj, M.bound);
+  const float y = l4d_x01(__ldg(A.rays_o + 3 * ray + 1), __ldg(A.rays_d + 3 * ray + 1), zj, M.bound);
+  const float z = l4d_x01(__ldg(A.rays_o + 3 * ray + 2), __ldg(A.rays_d + 3 * ray + 2), zj, M.bound);
+  float flow[6], dflow[6];
 #pragma unroll
-    for (int k = 0; k < 6; ++k) flow[k] = A.sv.flow[(size_t)k * P + p];
-    DfeatFromTile df{A.sv.dfeat + l4d_dfeat_off(A.sv, ray, j), active};
-    const uint32_t fi = l4d_frame_of<MF>(A.FT, ray);
-    l4d_bw_scatter_t<true, DfeatFromTile, false, true>(M, A.FT.frames[fi], A.G, x, y, z, flow, df, dflow, active, (int)ray, fi,
-                                                       fi * A.con_fstride, fi * A.comb_fstride);
-    if (active) {
+  for (int k = 0; k < 6; ++k) flow[k] = A.sv.flow[(size_t)k * P + p];
+  DfeatFromTile df{A.sv.dfeat + l4d_dfeat_off(A.sv, ray, j), active};
+  const uint32_t fi = l4d_frame_of<MF>(A.FT, ray);
+  l4d_bw_scatter_t<true, DfeatFromTile, false, true>(M, A.FT.frames[fi], A.G, x, y, z, flow, df, dflow, active, (int)ray, fi,
+                                                     fi * A.con_fstride, fi * A.comb_fstride);
+  if (active) {
 #pragma unroll
-      for (int k = 0; k < 6; ++k) A.sv.dflow[(size_t)k * P + p] = dflow[k];
-    }
+    for (int k = 0; k < 6; ++k) A.sv.dflow[(size_t)k * P + p] = dflow[k];
   }
 }
 
@@ -517,71 +517,117 @@ __global__ void __launch_bounds__(NT, L4D_FLOWGRID_MIN_CTAS) k_bwd_flowgrid(cons
 }
 
 // -------------------------------------------------------------------------------------------
-// backward 2b: static-hash reductions, LEVEL-MAJOR.  The fp32 gradient of the static table is 8 MB per level
-// (134 MB at L=16, far more than the 50 MB L2): walking all levels per sample makes the reductions miss in L2.
-// Here every CTA sweeps the samples once per level, so the whole
-// chip works on one level at a time and its gradient slab stays L2-resident.
+// backward 2/3, static-hash work: reductions LEVEL-MAJOR, one (level, block of NT samples) per call.  The fp32 gradient of
+// the static table is 8 MB per level (134 MB at L=16, far more than the 50 MB L2): walking all levels per sample makes the
+// reductions miss in L2.  k_bwd_encoders hands these blocks out in level order, so the whole chip works on one level at a
+// time and its gradient slab stays L2-resident.
 // -------------------------------------------------------------------------------------------
-// The kernel's time follows the reductions it issues (H100: 31.1 ms at 112.6 RED.128 per sample, 35.2 ms at 128).
+// As a kernel of its own (k_bwd_scatter_static), its time followed the reductions it issues (H100: 31.1 ms at 112.6 RED.128
+// per sample, 35.2 ms at 128).
 // L4D_STATIC_VERTEX_RUNS (default 1): every level goes through l4d_static_vertex_scatter_warp: at the coarse levels (0-7 at
 // L = 16) consecutive samples share cells or corners, and each distinct vertex of a warp gets one RED (97.4 per sample on the
 // benchmark's rays, scripts/red_count.py); at the fine levels one ballot finds no shared vertex and the lanes issue their 8
 // corners.  0 selects the former path, kept as the A/B reference while the step-time effect under a power cap is open (DESIGN.md
 // 9, item 4): runs of equal cells (l4d_static_scatter_warp) at the levels up to res L4D_STATIC_AGG_RES (113.4 REDs per sample;
 // bench.py::red_counts models this path), per-lane REDs above.
-// H100 80GB HBM3 at a 400 W power limit, L = 16, ms per launch of 16,384 rays: former path at res 1200 and bound 5 (54
-// registers, 9 CTAs/SM resident, no spills) 31.1-31.7, at bound 12 (40 registers, 16 B of spills) 33.4, at 16 (32, 56 B) 40.7,
-// aggregation off at bound 12 (40, no spills) 35.2; vertex runs at bound 4 (96 registers, no spills) 27.4, 5 (94, no spills)
-// 27.1-27.5, 6 (80, 60 B of spill stores) 31.2, 8 (64, 136 B) not run -> 5 either way.
+// The kernel of its own, H100 80GB HBM3 at a 400 W power limit, L = 16, ms per launch of 16,384 rays: former path at res 1200
+// and bound 5 (54 registers, 9 CTAs/SM resident, no spills) 31.1-31.7, at bound 12 (40 registers, 16 B of spills) 33.4, at 16
+// (32, 56 B) 40.7, aggregation off at bound 12 (40, no spills) 35.2; vertex runs at bound 4 (96 registers, no spills) 27.4, 5
+// (94, no spills) 27.1-27.5, 6 (80, 60 B of spill stores) 31.2.  At 700 W, at one CTA per SM, 24.0 against 26.3 at five: the
+// reduction rate, not the CTA count, bounds it, which is what lets k_bwd_encoders give it a single CTA per SM.
 #ifndef L4D_STATIC_VERTEX_RUNS
 #define L4D_STATIC_VERTEX_RUNS 1
 #endif
 #ifndef L4D_STATIC_AGG_RES
 #define L4D_STATIC_AGG_RES 1200
 #endif
-#ifndef L4D_STATIC_SCATTER_MIN_CTAS
-#define L4D_STATIC_SCATTER_MIN_CTAS (L4D_STATIC_VERTEX_RUNS || L4D_STATIC_AGG_RES ? 5 : 8)
-#endif
 template <int NT>
-__global__ void __launch_bounds__(NT, L4D_STATIC_SCATTER_MIN_CTAS) k_bwd_scatter_static(const __grid_constant__ SplitArgs A) {
+__device__ __forceinline__ void l4d_static_scatter_block(const SplitArgs& A, int l, size_t base) {
   const DevModel& M = A.M;
   const size_t P = A.sv.P;
   const RaySampling rs = l4d_make_sampling(M.near_lidar, M.far_lidar, A.S, A.perturb, A.seed);
-  const int L = (int)M.gs.n_levels;
   const int row_hash_s = 2 * (int)M.n_scales * 8;
-#pragma unroll 1
-  for (int l = 0; l < L; ++l) {
-    float* gbase = A.G.hs + (size_t)M.gs.offset[l] * 4;
-    const size_t dk = l4d_dfeat_k(row_hash_s + 4 * l);     // row_hash_s is a multiple of 16: one float4 per level
-    for (size_t base = (size_t)blockIdx.x * NT; base < P; base += (size_t)gridDim.x * NT) {
-      // whole warps stay together (the warp sinks shuffle); lanes past the end shadow the last sample with zero gradient
-      const size_t pp = base + threadIdx.x;
-      const bool active = pp < P;
-      const size_t p = active ? pp : P - 1;
-      const uint32_t ray = (uint32_t)(p / A.S), j = (uint32_t)(p % A.S);
-      float4 dd = __ldg(reinterpret_cast<const float4*>(A.sv.dfeat + l4d_dfeat_off(A.sv, ray, j) + dk));
-      if (!active) dd = make_float4(0.f, 0.f, 0.f, 0.f);
-      const float zj = l4d_z(rs, A.ray_offset + ray, j);
-      const float x = l4d_x01(__ldg(A.rays_o + 3 * ray), __ldg(A.rays_d + 3 * ray), zj, M.bound);
-      const float y = l4d_x01(__ldg(A.rays_o + 3 * ray + 1), __ldg(A.rays_d + 3 * ray + 1), zj, M.bound);
-      const float z = l4d_x01(__ldg(A.rays_o + 3 * ray + 2), __ldg(A.rays_d + 3 * ray + 2), zj, M.bound);
-      uint32_t idx[8]; float w[8];
-      l4d_corners3(M.gs, l, x, y, z, idx, w);
-      uint32_t cx, cy, cz; float fx, fy, fz;
-      const float sc = M.gs.scale[l];
-      l4d_pos_fract(sc, x, cx, fx); l4d_pos_fract(sc, y, cy, fy); l4d_pos_fract(sc, z, cz, fz);
+  float* gbase = A.G.hs + (size_t)M.gs.offset[l] * 4;
+  const size_t dk = l4d_dfeat_k(row_hash_s + 4 * l);     // row_hash_s is a multiple of 16: one float4 per level
+  // whole warps stay together (the warp sinks shuffle); lanes past the end shadow the last sample with zero gradient
+  const size_t pp = base + threadIdx.x;
+  const bool active = pp < P;
+  const size_t p = active ? pp : P - 1;
+  const uint32_t ray = (uint32_t)(p / A.S), j = (uint32_t)(p % A.S);
+  float4 dd = __ldg(reinterpret_cast<const float4*>(A.sv.dfeat + l4d_dfeat_off(A.sv, ray, j) + dk));
+  if (!active) dd = make_float4(0.f, 0.f, 0.f, 0.f);
+  const float zj = l4d_z(rs, A.ray_offset + ray, j);
+  const float x = l4d_x01(__ldg(A.rays_o + 3 * ray), __ldg(A.rays_d + 3 * ray), zj, M.bound);
+  const float y = l4d_x01(__ldg(A.rays_o + 3 * ray + 1), __ldg(A.rays_d + 3 * ray + 1), zj, M.bound);
+  const float z = l4d_x01(__ldg(A.rays_o + 3 * ray + 2), __ldg(A.rays_d + 3 * ray + 2), zj, M.bound);
+  uint32_t idx[8]; float w[8];
+  l4d_corners3(M.gs, l, x, y, z, idx, w);
+  uint32_t cx, cy, cz; float fx, fy, fz;
+  const float sc = M.gs.scale[l];
+  l4d_pos_fract(sc, x, cx, fx); l4d_pos_fract(sc, y, cy, fy); l4d_pos_fract(sc, z, cz, fz);
 #if L4D_STATIC_VERTEX_RUNS
-      const int cell[3] = {(int)cx, (int)cy, (int)cz};
-      l4d_static_vertex_scatter_warp(gbase, idx, w, dd, cell, (int)ray, active);
+  const int cell[3] = {(int)cx, (int)cy, (int)cz};
+  l4d_static_vertex_scatter_warp(gbase, idx, w, dd, cell, (int)ray, active);
 #else
-      if (L4D_STATIC_AGG_RES && M.gs.res[l] <= (uint32_t)L4D_STATIC_AGG_RES) {       // warp-uniform
-        // equal keys <=> equal cells for neighbouring lanes (their linear cell indices differ by far less than 2^32)
-        l4d_static_scatter_warp(gbase, idx, w, dd, (int)(cx + M.gs.res[l] * (cy + M.gs.res[l] * cz)));
-      } else if (active) {
+  if (L4D_STATIC_AGG_RES && M.gs.res[l] <= (uint32_t)L4D_STATIC_AGG_RES) {       // warp-uniform
+    // equal keys <=> equal cells for neighbouring lanes (their linear cell indices differ by far less than 2^32)
+    l4d_static_scatter_warp(gbase, idx, w, dd, (int)(cx + M.gs.res[l] * (cy + M.gs.res[l] * cz)));
+  } else if (active) {
 #pragma unroll
-        for (int c = 0; c < 8; ++c) l4d_red4(gbase + (size_t)idx[c] * 4, w[c] * dd.x, w[c] * dd.y, w[c] * dd.z, w[c] * dd.w);
-      }
+    for (int c = 0; c < 8; ++c) l4d_red4(gbase + (size_t)idx[c] * 4, w[c] * dd.x, w[c] * dd.y, w[c] * dd.z, w[c] * dd.w);
+  }
 #endif
+}
+
+// -------------------------------------------------------------------------------------------
+// backward 2/3: the encoder work and the static-hash work in one persistent launch.  The two are bound by different
+// units - the encoder work mostly by plane arithmetic, the static hash by the L2 reduction rate - so CTAs of both kinds
+// resident on one SM overlap them.  Each kind takes its blocks from a work-ticket counter (encoder: blocks of NT samples;
+// static hash: (level, block) in level-major order); a CTA whose own queue is empty drains the other one, so neither
+// kind idles while the other has work.  Blocks [0, n_static), L4D_SCATTER_STATIC_PER_SM per SM, start on the static queue:
+// the first wave is dispatched in block order, close to one CTA per SM at a time (at the benchmark's launch 116 of the 132
+// SMs got 3 encoder-first + 1 static-first CTAs, 8 got 2 + 2 and 8 got 4 + 0; the tickets balance the rest).
+// tickets: three zeroed counters in grad_work (encoder, static, CTAs done); the last CTA out zeroes them again.
+// H100 80GB HBM3 at a 700 W power limit, L = 16, ms per launch of 16,384 rays after six Adam steps: the two kinds as separate
+// kernels one after the other at full grids 23.5 + 26.3 = 49.8; on two streams at 3 + 1 CTAs/SM 40.9, at 2 + 2 47.4 -> one
+// static CTA per SM.  In the benchmark's profile pass this kernel takes 51.6 against 57.2 for the two separate kernels.
+// -------------------------------------------------------------------------------------------
+#ifndef L4D_SCATTER_STATIC_PER_SM
+#define L4D_SCATTER_STATIC_PER_SM 1
+#endif
+// the next ticket of counter c for the whole CTA
+__device__ __forceinline__ uint32_t l4d_cta_ticket(uint32_t* c, uint32_t& s_t) {
+  __syncthreads();                       // every thread has read the previous ticket
+  if (threadIdx.x == 0) s_t = atomicAdd(c, 1u);
+  __syncthreads();
+  return s_t;
+}
+template <int NT, bool MF>
+__global__ void __launch_bounds__(NT, L4D_SCATTER_MIN_CTAS) k_bwd_encoders(const __grid_constant__ SplitArgs A, uint32_t n_static) {
+  __shared__ uint32_t s_t;
+  uint32_t* tickets = A.scatter_tickets;
+  const uint32_t blocks = (uint32_t)((A.sv.P + NT - 1) / NT);
+  const uint32_t first = blockIdx.x < n_static ? 1u : 0u;          // queue 0: encoder blocks, 1: static-hash (level, block)
+#pragma unroll 1
+  for (uint32_t k = 0; k < 2; ++k) {
+    const uint32_t q = first ^ k;
+    const uint32_t n = q ? blocks * A.M.gs.n_levels : blocks;
+    uint32_t t = l4d_cta_ticket(tickets + q, s_t);
+    while (t < n) {
+      uint32_t next = 0;
+      if (threadIdx.x == 0) next = atomicAdd(tickets + q, 1u);      // drawn ahead: its latency hides under this block's work
+      if (q) l4d_static_scatter_block<NT>(A, (int)(t / blocks), (size_t)(t % blocks) * NT);
+      else l4d_encoder_scatter_block<NT, MF>(A, (size_t)t * NT);
+      __syncthreads();
+      if (threadIdx.x == 0) s_t = next;
+      __syncthreads();
+      t = s_t;
+    }
+  }
+  if (threadIdx.x == 0) {
+    __threadfence();                                                 // this CTA's draws come before its count
+    if (atomicAdd(tickets + 2, 1u) == gridDim.x - 1) {               // no CTA draws any more
+      tickets[0] = 0u; tickets[1] = 0u; tickets[2] = 0u;
     }
   }
 }

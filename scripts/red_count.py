@@ -1,6 +1,6 @@
 """Gradient updates per sample that the backward's hash-grid scatters send to L2, on the benchmark's own rays (host only).
 
-For the static hash (k_bwd_scatter_static) and the dynamic hash (k_bwd_scatter, contracted path: one float per entry), per level
+For the static hash and the dynamic hash (contracted path: one float per entry), both scattered by k_bwd_encoders, per level
 and in total, under three reductions of a warp of 32 consecutive samples of one ray:
   per-lane    every sample updates each of its corners (8 in 3D, 4 in 2D);
   cell-run    runs of consecutive samples in the same cell update each corner once (the former static-hash path used it at the
